@@ -85,7 +85,8 @@ static const char* launch_k_plan(const LtplLattice* lat, const LtplParams* prm, 
     if (smem > 200 * 1024) return "lattice window too large for shared memory";
     const bool zone = dm->n_zones > 0;
     const bool dense = lat->h.num_edges >= 2 * lat->h.num_nodes;   // in-edges per node (dp_run<.., DENSE>)
-    typedef void (*PlanFn)(const LatDev, const LtplParams, const LtplDims, const LtplBuffers, const int, const int, const int);
+    typedef void (*PlanFn)(const __grid_constant__ LatDev, const __grid_constant__ LtplParams, const __grid_constant__ LtplDims,
+                           const __grid_constant__ LtplBuffers, const int, const int, const int);
     static const PlanFn fns[8] = {k_plan<false, false, false>, k_plan<true, false, false>, k_plan<false, true, false>,
                                   k_plan<true, true, false>,   k_plan<false, false, true>, k_plan<true, false, true>,
                                   k_plan<false, true, true>,   k_plan<true, true, true>};

@@ -22,7 +22,7 @@ __host__ __device__ inline size_t emerg_smem_bytes_per_warp(int n_export) {
 }
 
 __global__ void __launch_bounds__(LTPL_WARPS_PER_CTA * 32)
-k_emergency(const LtplParams prm, const LtplDims dm, const LtplBuffers bf) {
+k_emergency(const __grid_constant__ LtplParams prm, const __grid_constant__ LtplDims dm, const __grid_constant__ LtplBuffers bf) {
     extern __shared__ __align__(16) unsigned char em_smem[];
     const int lane = threadIdx.x & 31;
     const int wib = threadIdx.x >> 5;

@@ -27,7 +27,8 @@ __device__ __forceinline__ void enqueue_path(const LtplBuffers& bf, const LtplDi
 // STATE: stateful tick (ltpl_state.cuh): the constant part and the list prefixes come from the previous tick's buffers
 template <bool STATE>
 __global__ void __launch_bounds__(LTPL_WARPS_PER_CTA * 32, LTPL_PATH_MINB)
-k_path(const LatDev lt, const LtplParams prm, const LtplDims dm, const LtplBuffers bf) {
+k_path(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm,
+       const __grid_constant__ LtplDims dm, const __grid_constant__ LtplBuffers bf) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int lane = threadIdx.x & 31;
     const int wib = threadIdx.x >> 5;

@@ -38,7 +38,8 @@ __device__ __forceinline__ void head_curv(double ax1, double ax2, double ax3, do
 }
 
 __global__ void __launch_bounds__(LTPL_WARPS_PER_CTA * 32)
-k_startpos(const LatDev lt, const LtplParams prm, const LtplDims dm, const LtplBuffers bf) {
+k_startpos(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm,
+           const __grid_constant__ LtplDims dm, const __grid_constant__ LtplBuffers bf) {
     const int lane = threadIdx.x & 31;
     const int b = blockIdx.x * LTPL_WARPS_PER_CTA + (threadIdx.x >> 5);
     if (b >= dm.batch) return;
@@ -522,16 +523,24 @@ __device__ __forceinline__ int disc_pairs(const LatDev& lt, int o, int p_start, 
     return o;
 }
 
+// action-set table of k_plan packed into one integer: action a holds its name (LTPL_ACT_STRAIGHT .. LTPL_ACT_RIGHT) in
+// bits 5a .. 5a+2 and its filter in bits 5a+3 .. 5a+4
+__device__ __forceinline__ int act_entry(int a, int name, int filter) { return (name | filter << 3) << (5 * a); }
+__device__ __forceinline__ int act_name(int acts, int a) { return (acts >> (5 * a)) & 7; }
+__device__ __forceinline__ int act_filter(int acts, int a) { return (acts >> (5 * a + 3)) & 3; }
+
 #ifndef LTPL_PLAN_MINB
 #define LTPL_PLAN_MINB 8   // resident CTAs per SM the register allocation is held to (occupancy hides the L1/L2 latency;
-                           // H100 sweep in DESIGN.md section 5: 8 is the fastest of 6 / 8 / 10 / 12 on both lattices)
+                           // H100 sweep in DESIGN.md section 5: of 6 / 8 / 10 / 12 / 16, 8 gives the fastest k_plan on
+                           // both lattices; 10 ties it on the l216 tick)
 #endif
 // STATE: stateful tick (ltpl_state.cuh): start node / constant segment come from k_state, the constant segment lives in
 // the previous tick's path planes, pos_est and the last action id enter the action-set logic, the first edges of the
 // last solution are cheaper
 template <bool ZONE, bool STATE = false, bool DENSE = false>
 __global__ void __launch_bounds__(LTPL_WARPS_PER_CTA * 32, LTPL_PLAN_MINB)
-k_plan(const LatDev lt, const LtplParams prm, const LtplDims dm, const LtplBuffers bf, const int maxn, const int hl,
+k_plan(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm,
+       const __grid_constant__ LtplDims dm, const __grid_constant__ LtplBuffers bf, const int maxn, const int hl,
        const int mask_words) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int lane = threadIdx.x & 31;
@@ -765,31 +774,26 @@ k_plan(const LatDev lt, const LtplParams prm, const LtplDims dm, const LtplBuffe
     }
 
     // ---- action sets (MOPG:124-174); filter: 0 planning_range, 1 default, 2 overtake_left, 3 overtake_right ----
-    int n_act, names[3], filt[3];
+    // (one integer holds the table, see act_entry: a run-time indexed array would live in local memory)
+    int n_act, acts;
     if (obj_in_const || obj_beside) {
         n_act = 1;
-        names[0] = LTPL_ACT_FOLLOW;
-        filt[0] = 0;
+        acts = act_entry(0, LTPL_ACT_FOLLOW, 0);
         // last_action_id (MOPG:130): the executed action, 'emergency' already translated by k_state (st_info[0] = its slot)
         const int last_act = STATE ? bf.prev_action_id[bf.st_info[8 * (size_t)b]] : LTPL_ACT_STRAIGHT;
         if (!obj_in_const && (last_act == LTPL_ACT_LEFT || last_act == LTPL_ACT_RIGHT)) {   // MOPG:130-133: keep overtaking
-            names[1] = last_act;
-            filt[1] = 1;
+            acts |= act_entry(1, last_act, 1);
             n_act = 2;
         } else if (!obj_in_const) {  // last_action_id is the forced "straight" on the first tick -> offer left and right
-            names[1] = LTPL_ACT_LEFT;  filt[1] = 1;
-            names[2] = LTPL_ACT_RIGHT; filt[2] = 1;
+            acts |= act_entry(1, LTPL_ACT_LEFT, 1) | act_entry(2, LTPL_ACT_RIGHT, 1);
             n_act = 3;
         }
     } else if (closest_idx >= 0 && con_node >= 0) {
         n_act = 3;
-        names[0] = LTPL_ACT_FOLLOW; filt[0] = 0;
-        names[1] = LTPL_ACT_LEFT;   filt[1] = 2;
-        names[2] = LTPL_ACT_RIGHT;  filt[2] = 3;
+        acts = act_entry(0, LTPL_ACT_FOLLOW, 0) | act_entry(1, LTPL_ACT_LEFT, 2) | act_entry(2, LTPL_ACT_RIGHT, 3);
     } else {
         n_act = 1;
-        names[0] = LTPL_ACT_STRAIGHT;
-        filt[0] = 1;
+        acts = act_entry(0, LTPL_ACT_STRAIGHT, 1);
     }
 
     // ---- graph search per action (MOPG:188-257) ----
@@ -843,8 +847,8 @@ k_plan(const LatDev lt, const LtplParams prm, const LtplDims dm, const LtplBuffe
     int pair_reach = -1, pair_tie = 0;   // second search of an 'overtake_left' / 'overtake_right' pair (dp_run_pair)
     #pragma unroll 1
     for (int a = 0; a < n_act; ++a) {
-        int name = names[a];
-        const int f = filt[a];
+        int name = act_name(acts, a);
+        const int f = act_filter(acts, a);
         int rem_layer = -1, rem_lo = 0, rem_hi = 0;
         if (f == 2) {  // remove nodes [n_obj, n_l) of the object's layer (MOPG:148-152)
             rem_layer = con_layer;
@@ -872,7 +876,7 @@ k_plan(const LatDev lt, const LtplParams prm, const LtplDims dm, const LtplBuffe
             } else if (src == 2) {
                 reach = prev_reach;
             } else {
-                const bool with_next = (f == 2 && a + 1 < n_act && filt[a + 1] == 3);
+                const bool with_next = (f == 2 && a + 1 < n_act && act_filter(acts, a + 1) == 3);
                 if (f == 3 && pair_reach >= 0) {          // searched together with 'overtake_left' (dp_run_pair)
                     reach = pair_reach;
                     tie = pair_tie;
@@ -1019,7 +1023,7 @@ __host__ __device__ inline size_t table_smem_bytes_per_warp(int maxn, int hl) {
 }
 
 __global__ void __launch_bounds__(LTPL_WARPS_PER_CTA * 32)
-k_follow_table(const LatDev lt, const int maxn, int* tab_reach, unsigned char* tab_node, int* tab_edge) {
+k_follow_table(const __grid_constant__ LatDev lt, const int maxn, int* tab_reach, unsigned char* tab_node, int* tab_edge) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int lane = threadIdx.x & 31;
     const int wib = threadIdx.x >> 5;

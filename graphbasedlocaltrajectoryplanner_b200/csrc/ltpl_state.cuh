@@ -53,7 +53,8 @@ __device__ __forceinline__ int find_edge(const LatDev& lt, int layer, int src, i
 }
 
 __global__ void __launch_bounds__(LTPL_WARPS_PER_CTA * 32)
-k_state(const LatDev lt, const LtplParams prm, const LtplDims dm, const LtplBuffers bf) {
+k_state(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm,
+        const __grid_constant__ LtplDims dm, const __grid_constant__ LtplBuffers bf) {
     const int lane = threadIdx.x & 31;
     const int b = sub_scenario(dm, LTPL_WARPS_PER_CTA);
     if (b < 0) return;
@@ -226,7 +227,8 @@ __device__ __forceinline__ void ref_obj_dist(const LtplDims& dm, const LtplBuffe
 // k_ref: get_ref_idx (OTH:518-601) + follow-mode object distance (OTH:774-784)
 // ---------------------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(LTPL_WARPS_PER_CTA * 32)
-k_ref(const LatDev lt, const LtplParams prm, const LtplDims dm, const LtplBuffers bf) {
+k_ref(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm,
+      const __grid_constant__ LtplDims dm, const __grid_constant__ LtplBuffers bf) {
     const int lane = threadIdx.x & 31;
     const int b = sub_scenario(dm, LTPL_WARPS_PER_CTA);
     if (b < 0) return;
@@ -339,7 +341,7 @@ k_ref(const LatDev lt, const LtplParams prm, const LtplDims dm, const LtplBuffer
 // One warp per path.
 // ---------------------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(LTPL_WARPS_PER_CTA * 32)
-k_prefix(const LtplDims dm, const LtplBuffers bf) {
+k_prefix(const __grid_constant__ LtplDims dm, const __grid_constant__ LtplBuffers bf) {
     const int lane = threadIdx.x & 31;
     const int B = dm.batch;
     const int q = sub_path(dm, LTPL_WARPS_PER_CTA);
@@ -383,7 +385,7 @@ k_prefix(const LtplDims dm, const LtplBuffers bf) {
 // the velocity kernel and k_prefix (which adds vel_course, the arc-length offset and the row count as for every path).
 // ---------------------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(LTPL_WARPS_PER_CTA * 32)
-k_backup(const LtplParams prm, const LtplDims dm, const LtplBuffers bf) {
+k_backup(const __grid_constant__ LtplParams prm, const __grid_constant__ LtplDims dm, const __grid_constant__ LtplBuffers bf) {
     const int lane = threadIdx.x & 31;
     const int b = sub_scenario(dm, LTPL_WARPS_PER_CTA);
     if (b < 0) return;

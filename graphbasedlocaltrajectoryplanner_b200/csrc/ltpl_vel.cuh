@@ -30,7 +30,7 @@ __device__ __forceinline__ double acc_brake(double w, double kabs, double ax_max
 
 // (P, 7) rows s, x, y, psi, kappa, vx, ax of every kept trajectory, cut to nmbr_export_points (OTH:941, LTPL:401-406)
 __global__ void __launch_bounds__(LTPL_WARPS_PER_CTA_EXPORT * 32)
-k_export(const LtplDims dm, const LtplBuffers bf) {
+k_export(const __grid_constant__ LtplDims dm, const __grid_constant__ LtplBuffers bf) {
     const int B = dm.batch;
     const int lane = threadIdx.x & 31;
     const int q = sub_path(dm, LTPL_WARPS_PER_CTA_EXPORT);   // a path of this launch's window ...

@@ -394,6 +394,7 @@ __device__ __forceinline__ void vr_convert_el(float* X0, float* X4, double* s_ou
 // warp roles (other class | follow warp 0 | follow warp 1) share one loop, so the kernel stays small in the instruction
 // cache although six different profiles pass through it.
 // GG: location dependent local_gg (buffers.gg, OTH:649-666): one more row per path (AX)
+// No __grid_constant__ here: no parameter is copied to local memory, and with it the H100 timing is 2-4 % slower.
 template <bool STATE, bool EXP1, bool GG>
 __global__ void __launch_bounds__(VR_THREADS, 7)
 k_vel_res(const LatDev lt, const LtplParams prm, const LtplDims dm, const LtplBuffers bf, const int nmax) {

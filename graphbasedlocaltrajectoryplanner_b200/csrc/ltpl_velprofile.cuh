@@ -73,7 +73,7 @@ __device__ __forceinline__ void vd_store_w(const float* tile, float* base, int p
 
 template <bool EXP1>
 __global__ void __launch_bounds__(32)
-k_velprofile(const LtplParams prm, const LtplVelBatch vb) {
+k_velprofile(const __grid_constant__ LtplParams prm, const __grid_constant__ LtplVelBatch vb) {
     extern __shared__ __align__(16) unsigned char vd_smem[];
     double* t_k = reinterpret_cast<double*>(vd_smem);
     double* t_e = t_k + VD_TILE;
