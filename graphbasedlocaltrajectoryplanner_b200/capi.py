@@ -12,7 +12,7 @@ import os
 import subprocess
 import sys
 
-ABI_VERSION = 12
+ABI_VERSION = 13
 MAX_SUB = 8
 NSLOT = 3
 KMAX = 16
@@ -61,7 +61,7 @@ class Params(C.Structure):
                 ("dyn_model_exp", C.c_double), ("drag_coeff", C.c_double), ("m_veh", C.c_double),
                 ("vel_max", C.c_double), ("gg_scale", C.c_double), ("gg_ax", C.c_double), ("gg_ay", C.c_double),
                 ("safety_d", C.c_double), ("n_axm", C.c_int32), ("traj_base_id", C.c_int32),
-                ("incl_emerg_traj", C.c_int32), ("pad0", C.c_int32), ("delaycomp", C.c_double),
+                ("incl_emerg_traj", C.c_int32), ("filt_window", C.c_int32), ("delaycomp", C.c_double),
                 ("w_last_edges", C.c_double * 4),
                 ("axm_v", C.c_double * MAX_AXM), ("axm_a", C.c_double * MAX_AXM), ("axm_s", C.c_double * MAX_AXM)]
 

@@ -18,6 +18,7 @@
 #include "ltpl_velprofile.cuh"
 #include "ltpl_emerg.cuh"
 #include "ltpl_state.cuh"
+#include "ltpl_smooth.cuh"
 
 static std::atomic<unsigned long long> g_launches{0};
 
@@ -329,6 +330,8 @@ static int check_common(const LtplLattice* lat, const LtplParams* prm, const Ltp
         return fail("dims.n_zones > 0 needs buffers.zone_bits, buffers.zone_sel and dims.n_zone_words");
     if (prm->axm_v[prm->n_axm - 1] < prm->vel_max)  // tph.calc_vel_profile input check
         return fail("ax_max_machines has to cover the entire velocity range of the car (i.e. >= v_max)!");
+    if (prm->filt_window < 0 || (prm->filt_window > 1 && prm->filt_window % 2 == 0))   // tph.conv_filt input check
+        return fail("params.filt_window: window width of moving average filter must be odd (0 or 1: no smoothing)");
     return 0;
 }
 
@@ -386,10 +389,21 @@ static int launch_emergency(const LtplParams* prm, const LtplDims* w, const Ltpl
 static const char* kVelCapacity =
     "k_vel: dims.p_max exceeds the shared-memory capacity of the velocity kernel (<= 512, % 4 == 0)";
 
-// one scenario window of calc_vel_profile.  First tick: k_vel_res (exports its rows itself) (-> k_emergency).
-// Stateful tick: k_ref -> k_vel_res -> k_backup -> k_prefix -> k_export (-> k_emergency)
+// velocity smoothing of every kept profile (params.filt_window > 1); a first tick also rewrites vx, ax of its export rows
+static int launch_smooth(const LtplParams* prm, const LtplDims* w, const LtplBuffers* bf, cudaStream_t st, bool stateful) {
+    const size_t smem = smooth_smem_bytes_per_warp(w->p_max) * LTPL_WARPS_PER_CTA;
+    if (smem > 48 * 1024) return fail("dims.p_max too large for k_smooth");
+    const int nq = LTPL_NSLOT * w->sub_cnt;
+    k_smooth<<<(nq + LTPL_WARPS_PER_CTA - 1) / LTPL_WARPS_PER_CTA, LTPL_WARPS_PER_CTA * 32, smem, st>>>(
+        *w, *bf, prm->filt_window, stateful ? 0 : 1);
+    return check_launch("k_smooth");
+}
+
+// one scenario window of calc_vel_profile.  First tick: k_vel_res (exports its rows itself) (-> k_smooth) (-> k_emergency).
+// Stateful tick: k_ref -> k_vel_res -> k_backup -> k_prefix (-> k_smooth) -> k_export (-> k_emergency)
 static int vel_window(const LtplLattice* lat, const LtplParams* prm, const LtplDims* w, const LtplBuffers* bf,
                       cudaStream_t st, bool stateful) {
+    const bool smooth = prm->filt_window > 1;
     const int grid_b = (w->sub_cnt + LTPL_WARPS_PER_CTA - 1) / LTPL_WARPS_PER_CTA;
     const int nq = LTPL_NSLOT * w->sub_cnt;
     const int grid_q = (nq + LTPL_WARPS_PER_CTA - 1) / LTPL_WARPS_PER_CTA;
@@ -404,9 +418,13 @@ static int vel_window(const LtplLattice* lat, const LtplParams* prm, const LtplD
         if (int r = check_launch("k_backup")) return r;
         k_prefix<<<grid_q, LTPL_WARPS_PER_CTA * 32, 0, st>>>(*w, *bf);
         if (int r = check_launch("k_prefix")) return r;
+        if (smooth)
+            if (int r = launch_smooth(prm, w, bf, st, true)) return r;
         k_export<<<(nq + LTPL_WARPS_PER_CTA_EXPORT - 1) / LTPL_WARPS_PER_CTA_EXPORT, LTPL_WARPS_PER_CTA_EXPORT * 32, 0,
                    st>>>(*w, *bf);
         if (int r = check_launch("k_export")) return r;
+    } else if (smooth) {
+        if (int r = launch_smooth(prm, w, bf, st, false)) return r;
     }
     if (prm->incl_emerg_traj) return launch_emergency(prm, w, bf, st);
     return 0;

@@ -26,6 +26,16 @@ from .scenarios import ScenarioBatch
 NSLOT = capi.NSLOT
 
 
+def check_filt_window(w) -> int:
+    """[SMOOTHING] filt_window_width: width of the moving-average window over every velocity profile (tph.conv_filt;
+    1 = no smoothing).  The reference raises on its first calc_vel_profile; here the value is refused up front."""
+    if int(w) != w or w < 1:
+        raise ValueError("filt_window_width must be a positive odd integer, got %r" % (w,))
+    if w % 2 != 1:
+        raise RuntimeError("Window width of moving average filter must be odd!")   # tph.conv_filt
+    return int(w)
+
+
 def read_online_config(path: str) -> dict:
     """online ini keys the batched path needs (reference: OTH:99-122, LTPL:168-173)."""
     cfg = configparser.ConfigParser()
@@ -39,7 +49,7 @@ def read_online_config(path: str) -> dict:
                 nmbr_export_points=json.loads(cfg.get('EXPORT', 'nmbr_export_points')),
                 v_max_offset=cfg.getfloat('ACTIONSET', 'v_max_offset'),
                 max_solutions=cfg.getint('ACTIONSET', 'max_solutions'),
-                filt_window_width=cfg.getint('SMOOTHING', 'filt_window_width'),
+                filt_window_width=check_filt_window(cfg.getint('SMOOTHING', 'filt_window_width')),
                 w_last_edges=json.loads(cfg.get('COST', 'w_last_edges')),
                 controller_type=ctype,
                 control_params=json.loads(cfg.get('FOLLOW', 'control_params_' + ctype)),
@@ -59,16 +69,15 @@ class BatchPlanner(object):
                  blob_tensor: torch.Tensor = None, stateful: bool = False):
         """``packed`` = (LatticeHeader, capacities) + ``blob_tensor`` (device uint8) when the blob arrived through a
         collective instead of being uploaded from ``lattice`` (parallel.broadcast_lattice)."""
+        self.online = dict(DEFAULT_ONLINE)
+        if online:
+            self.online.update(online)
+        self.online["filt_window_width"] = check_filt_window(self.online["filt_window_width"])
         self.lib = capi.load_library()
         if not torch.cuda.is_available():
             raise RuntimeError("BatchPlanner needs a CUDA device (H100, sm_90a); there is no CPU fallback")
         self.device = torch.device(device if device is not None else "cuda:0")
         torch.cuda.set_device(self.device)
-        self.online = dict(DEFAULT_ONLINE)
-        if online:
-            self.online.update(online)
-        if self.online["filt_window_width"] != 1:
-            raise NotImplementedError("velocity smoothing windows other than 1 (identity, shipped default) not batched")
         self.veh = dict(dyn_model_exp=float(veh_param_dyn_model_exp), drag_coeff=float(veh_param_dragcoeff),
                         m_veh=float(veh_param_mass))
         if packed is None:
@@ -149,6 +158,7 @@ class BatchPlanner(object):
         for i in range(3):
             p.w_last_edges[i] = float(o["w_last_edges"][i]) if i < len(o["w_last_edges"]) else 1.0
         p.incl_emerg_traj = 1 if incl_emerg_traj else 0
+        p.filt_window = int(o["filt_window_width"])
         for i in range(axm.shape[0]):
             p.axm_v[i] = axm[i, 0]
             p.axm_a[i] = axm[i, 1]

@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define LTPL_ABI_VERSION 12
+#define LTPL_ABI_VERSION 13
 
 /* action ids (OTH:14-17 ACTION_ID_MAP) */
 #define LTPL_ACT_NONE (-1)
@@ -155,7 +155,8 @@ typedef struct LtplParams {
     int32_t traj_base_id;        /* OTH:669 (+10 per calc_vel_profile call)           */
     int32_t incl_emerg_traj;     /* calc_vel_profile(incl_emerg_traj=True): append the brake-to-stop profile on the   */
                                  /* first kept trajectory of every scenario (OTH:1027-1034, calc_brake_emergency.py)   */
-    int32_t pad0;
+    int32_t filt_window;         /* SMOOTHING.filt_window_width: odd moving-average window over every kept velocity  */
+                                 /* profile (tph.conv_filt, OTH:926-941, 986-1004); 0 or 1 = no smoothing            */
     double delaycomp;            /* DELAY.delaycomp (OTH:117, 570)                    */
     double w_last_edges[4];      /* COST.w_last_edges, first three entries (GLNT:155-162); [3] unused */
     double axm_v[LTPL_MAX_AXM];

@@ -18,6 +18,16 @@ for tag in ("default", "l216"):
     pl.stage_scenarios(sc); pl.upload(); pl.set_startpos(); pl.tick()
     r = pl.records()
     print(tag, "trajectories:", sum(len(x.get("traj", {})) for x in r))
+# velocity smoothing (k_smooth): a first tick and a stateful tick at window 5, emergency trajectory on
+g = H.golden("ticks_default.npz")
+sc = make_scenarios(Track(H.TRACK_CSV), n, seed=78, n_obj_min=0, n_obj_max=3)
+ps = BatchPlanner(H.lattice_for("default"), online=dict(filt_window_width=5), device="cuda:0", stateful=True)
+ps.set_vel_params(ax_max_machines=g["ax_max_machines"], incl_emerg_traj=True, **VEL)
+ps.stage_scenarios(sc); ps.upload(); ps.set_startpos(); ps.tick()
+sel = ps.t["action_id"].max(dim=0).values.clamp(min=0).cpu().numpy()   # an action every scenario's tick returned
+ps.next_tick(sc, sel_action=sel, t_const=0.1)
+r = ps.records()
+print("smoothed stateful tick, trajectories:", sum(len(x.get("traj", {})) for x in r))
 mb = make_velocity_microbench(200, 150, seed=3)
 vx, ax = calc_vel_profile_batch(pl, mb["kappa"], mb["el"], mb["v_start"], mb["v_end"])
 print("dense vx mean", float(np.mean(vx)))
