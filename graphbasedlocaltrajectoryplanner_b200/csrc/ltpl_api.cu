@@ -7,10 +7,10 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <mutex>
 #include <new>
 #include <string>
 
-#define LTPL_WARPS_PER_CTA_EXPORT 8
 #include "ltpl_path.cuh"
 #include "ltpl_plan.cuh"
 #include "ltpl_vel.cuh"
@@ -21,41 +21,6 @@
 #include "ltpl_smooth.cuh"
 
 static std::atomic<unsigned long long> g_launches{0};
-
-// velocity kernel: one CTA per VR_P queued paths of one class, the paths resident in shared memory (ltpl_vel_res.cuh)
-static cudaError_t launch_k_vel(const LtplLattice* lat, const LtplParams* prm, const LtplDims* dm, const LtplBuffers* bf,
-                                cudaStream_t st, bool stateful = false) {
-    const int nq = LTPL_NSLOT * dm->sub_cnt;   // paths of this launch's scenario window
-    const int nmax = dm->p_max;
-    if (nmax > 32 * VR_MAXM || nmax % 4 != 0) return cudaErrorInvalidValue;
-    const bool gg = bf->gg != nullptr;   // location dependent local_gg: the general-exponent variant carries it
-    const size_t smem = vr_smem_bytes(nmax, gg);
-    if (smem > 200 * 1024) return cudaErrorInvalidValue;
-    static thread_local size_t attr_set = 0;
-    if (smem > attr_set) {
-        const void* fns[6] = {(const void*)k_vel_res<false, true, false>, (const void*)k_vel_res<true, true, false>,
-                              (const void*)k_vel_res<false, false, false>, (const void*)k_vel_res<true, false, false>,
-                              (const void*)k_vel_res<false, false, true>, (const void*)k_vel_res<true, false, true>};
-        for (const void* f : fns)
-            if (cudaError_t e = cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) return e;
-        attr_set = smem;
-    }
-    const int grid = nq / VR_P + 2;   // >= groups of the follow queue + groups of the other queue
-    const bool exp1 = prm->dyn_model_exp == 1.0 && !gg;
-    if (gg && stateful)
-        k_vel_res<true, false, true><<<grid, VR_THREADS, smem, st>>>(lat->d, *prm, *dm, *bf, nmax);
-    else if (gg)
-        k_vel_res<false, false, true><<<grid, VR_THREADS, smem, st>>>(lat->d, *prm, *dm, *bf, nmax);
-    else if (stateful && exp1)
-        k_vel_res<true, true, false><<<grid, VR_THREADS, smem, st>>>(lat->d, *prm, *dm, *bf, nmax);
-    else if (stateful)
-        k_vel_res<true, false, false><<<grid, VR_THREADS, smem, st>>>(lat->d, *prm, *dm, *bf, nmax);
-    else if (exp1)
-        k_vel_res<false, true, false><<<grid, VR_THREADS, smem, st>>>(lat->d, *prm, *dm, *bf, nmax);
-    else
-        k_vel_res<false, false, false><<<grid, VR_THREADS, smem, st>>>(lat->d, *prm, *dm, *bf, nmax);
-    return cudaSuccess;
-}
 
 static thread_local std::string g_err;
 
@@ -75,33 +40,91 @@ static int check_launch(const char* name) {
     return 0;
 }
 
+// CTAs of a launch with one warp per scenario / path
+static int ctas(int warps, int warps_per_cta = LTPL_WARPS_PER_CTA) { return (warps + warps_per_cta - 1) / warps_per_cta; }
+static const int kThreads = LTPL_WARPS_PER_CTA * 32;
 
-// k_plan<ZONE, STATE>: one warp per scenario (ltpl_plan.cuh)
-static const char* launch_k_plan(const LtplLattice* lat, const LtplParams* prm, const LtplDims* dm, const LtplBuffers* bf,
-                                 cudaStream_t st, bool stateful) {
+// Dynamic shared memory of a kernel family: a size above the 200 KB cap is refused, a size above the 48 KB default is
+// allowed by cudaFuncSetAttribute on every kernel of the family.  The attribute belongs to the kernel on the current
+// device and is shared by every handle and thread there, so it is only ever raised (another handle may rely on a larger
+// value), under a lock.  The size a handle has made sure of is kept per handle (one handle, one device) to skip the calls.
+enum SmemFamily { kSmemFollow, kSmemPlan, kSmemPath, kSmemVel };
+static std::mutex g_smem_lock;
+
+template <class Fn, size_t N>
+static int allow_smem(const LtplLattice* lat, SmemFamily fam, size_t smem, Fn const (&fns)[N], const char* name,
+                      const char* too_large) {
+    if (smem > 200 * 1024) return fail(too_large);
+    if (smem > 48 * 1024 && smem > lat->smem_allowed[fam]) {
+        std::lock_guard<std::mutex> lock(g_smem_lock);
+        for (Fn f : fns) {
+            cudaFuncAttributes a;
+            cudaError_t e = cudaFuncGetAttributes(&a, (const void*)f);
+            if (e == cudaSuccess && (size_t)a.maxDynamicSharedSizeBytes < smem)
+                e = cudaFuncSetAttribute((const void*)f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+            if (e != cudaSuccess) {
+                (void)cudaGetLastError();
+                g_err = std::string(name) + ": dynamic shared-memory attribute: " + cudaGetErrorString(e);
+                return -2;
+            }
+        }
+        lat->smem_allowed[fam] = smem;
+    }
+    return 0;
+}
+
+// k_plan<ZONE, STATE, DENSE>: one warp per scenario (ltpl_plan.cuh)
+static int launch_k_plan(const LtplLattice* lat, const LtplParams* prm, const LtplDims* dm, const LtplBuffers* bf,
+                         cudaStream_t st, bool stateful) {
     const int maxn = ((lat->h.max_nodes_per_layer + 31) / 32) * 32;
     const int hl = dm->h_max;
     const int mask_words = (lat->h.max_window_edges + 31) / 32 + 1;
     const size_t smem = plan_smem_bytes_per_warp(maxn, hl, mask_words) * LTPL_WARPS_PER_CTA;
-    if (smem > 200 * 1024) return "lattice window too large for shared memory";
-    const bool zone = dm->n_zones > 0;
-    const bool dense = lat->h.num_edges >= 2 * lat->h.num_nodes;   // in-edges per node (dp_run<.., DENSE>)
     typedef void (*PlanFn)(const __grid_constant__ LatDev, const __grid_constant__ LtplParams, const __grid_constant__ LtplDims,
                            const __grid_constant__ LtplBuffers, const int, const int, const int);
     static const PlanFn fns[8] = {k_plan<false, false, false>, k_plan<true, false, false>, k_plan<false, true, false>,
                                   k_plan<true, true, false>,   k_plan<false, false, true>, k_plan<true, false, true>,
                                   k_plan<false, true, true>,   k_plan<true, true, true>};
-    static thread_local size_t attr = 0;
-    if (smem > 48 * 1024 && smem > attr) {
-        for (PlanFn f : fns)
-            if (cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
-                return "cudaFuncSetAttribute(k_plan) failed";
-        attr = smem;
-    }
-    const int grid = (dm->sub_cnt + LTPL_WARPS_PER_CTA - 1) / LTPL_WARPS_PER_CTA, thr = LTPL_WARPS_PER_CTA * 32;
-    fns[(zone ? 1 : 0) + (stateful ? 2 : 0) + (dense ? 4 : 0)]<<<grid, thr, smem, st>>>(lat->d, *prm, *dm, *bf, maxn, hl,
-                                                                                        mask_words);
-    return nullptr;
+    if (int r = allow_smem(lat, kSmemPlan, smem, fns, "k_plan", "lattice window too large for shared memory")) return r;
+    const bool zone = dm->n_zones > 0;
+    const bool dense = lat->h.num_edges >= 2 * lat->h.num_nodes;   // in-edges per node (dp_run<.., DENSE>)
+    fns[(zone ? 1 : 0) + (stateful ? 2 : 0) + (dense ? 4 : 0)]<<<ctas(dm->sub_cnt), kThreads, smem, st>>>(
+        lat->d, *prm, *dm, *bf, maxn, hl, mask_words);
+    return check_launch("k_plan");
+}
+
+// k_path<STATE>: one warp per path (ltpl_path.cuh)
+static int launch_k_path(const LtplLattice* lat, const LtplParams* prm, const LtplDims* dm, const LtplBuffers* bf,
+                         cudaStream_t st, bool stateful) {
+    const size_t smem = path_smem_bytes_per_warp(dm->h_max) * LTPL_WARPS_PER_CTA;
+    typedef void (*PathFn)(const __grid_constant__ LatDev, const __grid_constant__ LtplParams,
+                           const __grid_constant__ LtplDims, const __grid_constant__ LtplBuffers);
+    static const PathFn fns[2] = {k_path<false>, k_path<true>};
+    if (int r = allow_smem(lat, kSmemPath, smem, fns, "k_path", "lattice window too large for shared memory")) return r;
+    fns[stateful]<<<ctas(LTPL_NSLOT * dm->sub_cnt), kThreads, smem, st>>>(lat->d, *prm, *dm, *bf);
+    return check_launch("k_path");
+}
+
+// velocity kernel: one CTA per VR_P queued paths of one class, the paths resident in shared memory (ltpl_vel_res.cuh)
+static int launch_k_vel(const LtplLattice* lat, const LtplParams* prm, const LtplDims* dm, const LtplBuffers* bf,
+                        cudaStream_t st, bool stateful) {
+    const int nmax = dm->p_max;
+    if (nmax > 32 * VR_MAXM)
+        return fail("k_vel: dims.p_max exceeds the shared-memory capacity of the velocity kernel (<= 512)");
+    const bool gg = bf->gg != nullptr;   // location dependent local_gg: the general-exponent variant carries it
+    const size_t smem = vr_smem_bytes(nmax, gg);
+    typedef void (*VelFn)(const LatDev, const LtplParams, const LtplDims, const LtplBuffers, const int);
+    // <STATE, EXP1, GG>: [stateful + 2 * (0 exponent 1, 1 general exponent, 2 local_gg planes)]
+    static const VelFn fns[6] = {k_vel_res<false, true, false>, k_vel_res<true, true, false>,
+                                 k_vel_res<false, false, false>, k_vel_res<true, false, false>,
+                                 k_vel_res<false, false, true>, k_vel_res<true, false, true>};
+    if (int r = allow_smem(lat, kSmemVel, smem, fns, "k_vel", "dims.p_max too large for the velocity kernel's shared memory"))
+        return r;
+    const int kind = gg ? 2 : (prm->dyn_model_exp == 1.0 ? 0 : 1);
+    const int nq = LTPL_NSLOT * dm->sub_cnt;   // paths of this launch's scenario window
+    const int grid = nq / VR_P + 2;            // >= groups of the follow queue + groups of the other queue
+    fns[(stateful ? 1 : 0) + 2 * kind]<<<grid, VR_THREADS, smem, st>>>(lat->d, *prm, *dm, *bf, nmax);
+    return check_launch("k_vel");
 }
 
 extern "C" {
@@ -199,19 +222,14 @@ int ltpl_lattice_create(const LtplLatticeHeader* h, void* dev_blob, LtplLattice*
     {  // follow table: one warp per node (k_follow_table), once per lattice
         const int maxn = ((h->max_nodes_per_layer + 31) / 32) * 32;
         const size_t smem = table_smem_bytes_per_warp(maxn, h->tab_stride) * LTPL_WARPS_PER_CTA;
-        cudaError_t e = cudaSuccess;
-        if (smem > 200 * 1024) {
+        if (int r = allow_smem(lat, kSmemFollow, smem, {k_follow_table}, "k_follow_table",
+                               "ltpl_lattice_create: planning range too large for shared memory")) {
             delete lat;
-            return fail("ltpl_lattice_create: planning range too large for shared memory");
+            return r;
         }
-        if (smem > 48 * 1024)
-            e = cudaFuncSetAttribute(k_follow_table, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e == cudaSuccess) {
-            k_follow_table<<<(h->num_nodes + LTPL_WARPS_PER_CTA - 1) / LTPL_WARPS_PER_CTA, LTPL_WARPS_PER_CTA * 32, smem>>>(
-                d, maxn, reinterpret_cast<int*>(p + h->off_tab_reach), p + h->off_tab_node,
-                reinterpret_cast<int*>(p + h->off_tab_edge));
-            e = cudaGetLastError();
-        }
+        k_follow_table<<<ctas(h->num_nodes), kThreads, smem>>>(d, maxn, reinterpret_cast<int*>(p + h->off_tab_reach),
+                                                              p + h->off_tab_node, reinterpret_cast<int*>(p + h->off_tab_edge));
+        cudaError_t e = cudaGetLastError();
         if (e == cudaSuccess) e = cudaDeviceSynchronize();
         if (e != cudaSuccess) {
             g_err = std::string("ltpl_lattice_create: k_follow_table: ") + cudaGetErrorString(e);
@@ -312,7 +330,9 @@ static int for_windows(const LtplLattice* lat, const LtplDims* dm, cudaStream_t 
 }
 }  // extern "C++"
 
-static int check_common(const LtplLattice* lat, const LtplParams* prm, const LtplDims* dm, const LtplBuffers* bf) {
+// every condition a call of the tick protocol checks; `stateful`: a tick with the iterative memory (ltpl_next_*)
+static int validate(const LtplLattice* lat, const LtplParams* prm, const LtplDims* dm, const LtplBuffers* bf,
+                    bool stateful) {
     if (!lat || !prm || !dm || !bf) return fail("null argument");
     if (dm->batch <= 0) return fail("dims.batch must be > 0");
     {   // every buffer in front of the optional block (zones, emergency, predictions) is required
@@ -332,170 +352,8 @@ static int check_common(const LtplLattice* lat, const LtplParams* prm, const Ltp
         return fail("ax_max_machines has to cover the entire velocity range of the car (i.e. >= v_max)!");
     if (prm->filt_window < 0 || (prm->filt_window > 1 && prm->filt_window % 2 == 0))   // tph.conv_filt input check
         return fail("params.filt_window: window width of moving average filter must be odd (0 or 1: no smoothing)");
-    return 0;
-}
-
-int ltpl_set_startpos_batch(const LtplLattice* lat, const LtplParams* prm, const LtplDims* dm, const LtplBuffers* bf,
-                            void* stream) {
-    if (int r = check_common(lat, prm, dm, bf)) return r;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const int grid = (dm->batch + LTPL_WARPS_PER_CTA - 1) / LTPL_WARPS_PER_CTA;
-    k_startpos<<<grid, LTPL_WARPS_PER_CTA * 32, 0, st>>>(lat->d, *prm, *dm, *bf);
-    return check_launch("k_startpos");
-}
-
-static const int kCntInts = 4 + 4 * LTPL_MAX_SUB;   // buffers.queue_cnt
-
-static int prepare_path_attr(const LtplDims* dm, bool stateful, size_t* smem_out) {
-    const size_t smem_path = path_smem_bytes_per_warp(dm->h_max) * LTPL_WARPS_PER_CTA;
-    if (smem_path > 200 * 1024) return fail("lattice window too large for shared memory");
-    static thread_local size_t attr_path[2] = {0, 0};
-    if (smem_path > 48 * 1024 && smem_path > attr_path[stateful]) {
-        const cudaError_t e = stateful ? cudaFuncSetAttribute(k_path<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_path)
-                                       : cudaFuncSetAttribute(k_path<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_path);
-        if (e != cudaSuccess) return fail("cudaFuncSetAttribute(k_path) failed");
-        attr_path[stateful] = smem_path;
-    }
-    *smem_out = smem_path;
-    return 0;
-}
-
-// one scenario window of calc_paths: (k_state ->) k_plan -> k_path
-static int paths_window(const LtplLattice* lat, const LtplParams* prm, const LtplDims* w, const LtplBuffers* bf,
-                        cudaStream_t st, bool stateful, size_t smem_path) {
-    const int grid_b = (w->sub_cnt + LTPL_WARPS_PER_CTA - 1) / LTPL_WARPS_PER_CTA;
-    const int grid_q = (LTPL_NSLOT * w->sub_cnt + LTPL_WARPS_PER_CTA - 1) / LTPL_WARPS_PER_CTA;
-    if (stateful) {
-        k_state<<<grid_b, LTPL_WARPS_PER_CTA * 32, 0, st>>>(lat->d, *prm, *w, *bf);
-        if (int r = check_launch("k_state")) return r;
-    }
-    if (const char* e = launch_k_plan(lat, prm, w, bf, st, stateful)) return fail(e);
-    if (int r = check_launch("k_plan")) return r;
-    if (stateful)
-        k_path<true><<<grid_q, LTPL_WARPS_PER_CTA * 32, smem_path, st>>>(lat->d, *prm, *w, *bf);
-    else
-        k_path<false><<<grid_q, LTPL_WARPS_PER_CTA * 32, smem_path, st>>>(lat->d, *prm, *w, *bf);
-    return check_launch("k_path");
-}
-
-static int launch_emergency(const LtplParams* prm, const LtplDims* w, const LtplBuffers* bf, cudaStream_t st) {
-    const size_t smem = emerg_smem_bytes_per_warp(w->n_export) * LTPL_WARPS_PER_CTA;
-    if (smem > 48 * 1024) return fail("n_export too large for k_emergency");
-    k_emergency<<<(w->sub_cnt + LTPL_WARPS_PER_CTA - 1) / LTPL_WARPS_PER_CTA, LTPL_WARPS_PER_CTA * 32, smem, st>>>(
-        *prm, *w, *bf);
-    return check_launch("k_emergency");
-}
-
-static const char* kVelCapacity =
-    "k_vel: dims.p_max exceeds the shared-memory capacity of the velocity kernel (<= 512, % 4 == 0)";
-
-// velocity smoothing of every kept profile (params.filt_window > 1); a first tick also rewrites vx, ax of its export rows
-static int launch_smooth(const LtplParams* prm, const LtplDims* w, const LtplBuffers* bf, cudaStream_t st, bool stateful) {
-    const size_t smem = smooth_smem_bytes_per_warp(w->p_max) * LTPL_WARPS_PER_CTA;
-    if (smem > 48 * 1024) return fail("dims.p_max too large for k_smooth");
-    const int nq = LTPL_NSLOT * w->sub_cnt;
-    k_smooth<<<(nq + LTPL_WARPS_PER_CTA - 1) / LTPL_WARPS_PER_CTA, LTPL_WARPS_PER_CTA * 32, smem, st>>>(
-        *w, *bf, prm->filt_window, stateful ? 0 : 1);
-    return check_launch("k_smooth");
-}
-
-// one scenario window of calc_vel_profile.  First tick: k_vel_res (exports its rows itself) (-> k_smooth) (-> k_emergency).
-// Stateful tick: k_ref -> k_vel_res -> k_backup -> k_prefix (-> k_smooth) -> k_export (-> k_emergency)
-static int vel_window(const LtplLattice* lat, const LtplParams* prm, const LtplDims* w, const LtplBuffers* bf,
-                      cudaStream_t st, bool stateful) {
-    const bool smooth = prm->filt_window > 1;
-    const int grid_b = (w->sub_cnt + LTPL_WARPS_PER_CTA - 1) / LTPL_WARPS_PER_CTA;
-    const int nq = LTPL_NSLOT * w->sub_cnt;
-    const int grid_q = (nq + LTPL_WARPS_PER_CTA - 1) / LTPL_WARPS_PER_CTA;
-    if (stateful) {
-        k_ref<<<grid_b, LTPL_WARPS_PER_CTA * 32, 0, st>>>(lat->d, *prm, *w, *bf);
-        if (int r = check_launch("k_ref")) return r;
-    }
-    if (launch_k_vel(lat, prm, w, bf, st, stateful) != cudaSuccess) return fail(kVelCapacity);
-    if (int r = check_launch("k_vel")) return r;
-    if (stateful) {
-        k_backup<<<grid_b, LTPL_WARPS_PER_CTA * 32, 0, st>>>(*prm, *w, *bf);
-        if (int r = check_launch("k_backup")) return r;
-        k_prefix<<<grid_q, LTPL_WARPS_PER_CTA * 32, 0, st>>>(*w, *bf);
-        if (int r = check_launch("k_prefix")) return r;
-        if (smooth)
-            if (int r = launch_smooth(prm, w, bf, st, true)) return r;
-        k_export<<<(nq + LTPL_WARPS_PER_CTA_EXPORT - 1) / LTPL_WARPS_PER_CTA_EXPORT, LTPL_WARPS_PER_CTA_EXPORT * 32, 0,
-                   st>>>(*w, *bf);
-        if (int r = check_launch("k_export")) return r;
-    } else if (smooth) {
-        if (int r = launch_smooth(prm, w, bf, st, false)) return r;
-    }
-    if (prm->incl_emerg_traj) return launch_emergency(prm, w, bf, st);
-    return 0;
-}
-
-static int launch_paths(const LtplLattice* lat, const LtplParams* prm, const LtplDims* dm, const LtplBuffers* bf,
-                        cudaStream_t st, bool stateful) {
-    size_t smem_path = 0;
-    if (int r = prepare_path_attr(dm, stateful, &smem_path)) return r;
-    if (cudaMemsetAsync(bf->queue_cnt, 0, kCntInts * sizeof(int), st) != cudaSuccess) return fail("memset(queue_cnt) failed");
-    return for_windows(lat, dm, st, [&](const LtplDims* w, cudaStream_t s) {
-        return paths_window(lat, prm, w, bf, s, stateful, smem_path);
-    });
-}
-
-static int launch_vel(const LtplLattice* lat, const LtplParams* prm, const LtplDims* dm, const LtplBuffers* bf,
-                      cudaStream_t st, bool stateful) {
     if (prm->incl_emerg_traj && !bf->em_info) return fail("params.incl_emerg_traj needs buffers.em_info");
-    if (cudaMemsetAsync(bf->queue_cnt + 2, 0, sizeof(int), st) != cudaSuccess) return fail("memset(export count) failed");
-    if (int r = for_windows(lat, dm, st, [&](const LtplDims* w, cudaStream_t s) {
-            return vel_window(lat, prm, w, bf, s, stateful);
-        }))
-        return r;
-    // stateful tick without an emergency trajectory: the next one must not take a stale one for executed (k_state)
-    if (stateful && !prm->incl_emerg_traj && bf->em_info &&
-        cudaMemsetAsync(bf->em_info, 0xFF, sizeof(int) * 3 * (size_t)dm->batch, st) != cudaSuccess)
-        return fail("memset(em_info) failed");
-    return 0;
-}
-
-// calc_paths + calc_vel_profile of one tick: every window runs its whole chain on its stream, one fork / join
-static int launch_tick(const LtplLattice* lat, const LtplParams* prm, const LtplDims* dm, const LtplBuffers* bf,
-                       cudaStream_t st, bool stateful) {
-    size_t smem_path = 0;
-    if (int r = prepare_path_attr(dm, stateful, &smem_path)) return r;
-    if (prm->incl_emerg_traj && !bf->em_info) return fail("params.incl_emerg_traj needs buffers.em_info");
-    if (cudaMemsetAsync(bf->queue_cnt, 0, kCntInts * sizeof(int), st) != cudaSuccess) return fail("memset(queue_cnt) failed");
-    if (int r = for_windows(lat, dm, st, [&](const LtplDims* w, cudaStream_t s) {
-            if (int r2 = paths_window(lat, prm, w, bf, s, stateful, smem_path)) return r2;
-            return vel_window(lat, prm, w, bf, s, stateful);
-        }))
-        return r;
-    if (stateful && !prm->incl_emerg_traj && bf->em_info &&
-        cudaMemsetAsync(bf->em_info, 0xFF, sizeof(int) * 3 * (size_t)dm->batch, st) != cudaSuccess)
-        return fail("memset(em_info) failed");
-    return 0;
-}
-
-int ltpl_calc_paths_batch(const LtplLattice* lat, const LtplParams* prm, const LtplDims* dm, const LtplBuffers* bf,
-                          void* stream) {
-    if (int r = check_common(lat, prm, dm, bf)) return r;
-    return launch_paths(lat, prm, dm, bf, static_cast<cudaStream_t>(stream), false);
-}
-
-int ltpl_calc_vel_profile_batch(const LtplLattice* lat, const LtplParams* prm, const LtplDims* dm,
-                                const LtplBuffers* bf, void* stream) {
-    if (int r = check_common(lat, prm, dm, bf)) return r;
-    return launch_vel(lat, prm, dm, bf, static_cast<cudaStream_t>(stream), false);
-}
-
-int ltpl_tick_batch(const LtplLattice* lat, const LtplParams* prm, const LtplDims* dm, const LtplBuffers* bf,
-                    void* stream) {
-    if (int r = check_common(lat, prm, dm, bf)) return r;
-    return launch_tick(lat, prm, dm, bf, static_cast<cudaStream_t>(stream), false);
-}
-
-// stateful tick (ltpl_state.cuh):
-//   ltpl_next_calc_paths_batch        k_state -> k_plan<.., true> -> k_path<true>
-//   ltpl_next_calc_vel_profile_batch  k_ref -> k_vel_res<true> -> k_backup -> k_prefix -> k_export
-static int check_stateful(const LtplLattice* lat, const LtplParams* prm, const LtplDims* dm, const LtplBuffers* bf) {
-    if (int r = check_common(lat, prm, dm, bf)) return r;
+    if (!stateful) return 0;
     if (!bf->prev_path || !bf->prev_path_len || !bf->prev_node_idx || !bf->prev_nodes || !bf->prev_n_nodes ||
         !bf->prev_coeff || !bf->prev_s_vx_ax || !bf->prev_action_id || !bf->prev_traj_len || !bf->prev_trim ||
         !bf->sel_action || !bf->pos_last || !bf->t_const || !bf->st_info || !bf->trim || !bf->vel_plan || !bf->course ||
@@ -503,60 +361,162 @@ static int check_stateful(const LtplLattice* lat, const LtplParams* prm, const L
         return fail("stateful tick: the buffers prev_*, sel_action, pos_last, t_const, st_info, trim, vel_plan, course, "
                     "obj_dist must be set");
     if (dm->n_zones > 0 && !bf->zone_s0) return fail("stateful tick with zones: buffers.zone_s0 must be set");
-    if (prm->incl_emerg_traj && !bf->em_info) return fail("params.incl_emerg_traj needs buffers.em_info");
     if (prm->delaycomp <= 0.0) return fail("params.delaycomp must be > 0");
     return 0;
 }
 
+int ltpl_set_startpos_batch(const LtplLattice* lat, const LtplParams* prm, const LtplDims* dm, const LtplBuffers* bf,
+                            void* stream) {
+    if (int r = validate(lat, prm, dm, bf, false)) return r;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    // a new session on a buffer set with memory: its first tick processes the zones anew (GLNT:43-77)
+    if (bf->trim && bf->zone_s0 && cudaMemsetAsync(bf->zone_s0, 0xFF, sizeof(int) * (size_t)dm->batch, st) != cudaSuccess)
+        return fail("memset(zone_s0) failed");
+    k_startpos<<<ctas(dm->batch), kThreads, 0, st>>>(lat->d, *prm, *dm, *bf);
+    return check_launch("k_startpos");
+}
+
+// buffers.queue_cnt: the path stage starts every count at 0, the velocity stage the export count [2]
+static int reset_counts(const LtplBuffers* bf, bool paths, cudaStream_t st) {
+    const size_t n = paths ? 4 + 4 * LTPL_MAX_SUB : 1;
+    if (cudaMemsetAsync(paths ? bf->queue_cnt : bf->queue_cnt + 2, 0, n * sizeof(int), st) != cudaSuccess)
+        return fail("memset(queue_cnt) failed");
+    return 0;
+}
+
+static int launch_export(const LtplDims* w, const LtplBuffers* bf, cudaStream_t st) {
+    k_export<<<ctas(LTPL_NSLOT * w->sub_cnt, LTPL_WARPS_PER_CTA_EXPORT), LTPL_WARPS_PER_CTA_EXPORT * 32, 0, st>>>(*w, *bf);
+    return check_launch("k_export");
+}
+
+static int launch_emergency(const LtplParams* prm, const LtplDims* w, const LtplBuffers* bf, cudaStream_t st) {
+    const size_t smem = emerg_smem_bytes_per_warp(w->n_export) * LTPL_WARPS_PER_CTA;
+    if (smem > 48 * 1024) return fail("n_export too large for k_emergency");
+    k_emergency<<<ctas(w->sub_cnt), kThreads, smem, st>>>(*prm, *w, *bf);
+    return check_launch("k_emergency");
+}
+
+// velocity smoothing of every kept profile (params.filt_window > 1); a first tick also rewrites vx, ax of its export rows
+static int launch_smooth(const LtplParams* prm, const LtplDims* w, const LtplBuffers* bf, cudaStream_t st, bool stateful) {
+    const size_t smem = smooth_smem_bytes_per_warp(w->p_max) * LTPL_WARPS_PER_CTA;
+    if (smem > 48 * 1024) return fail("dims.p_max too large for k_smooth");
+    k_smooth<<<ctas(LTPL_NSLOT * w->sub_cnt), kThreads, smem, st>>>(*w, *bf, prm->filt_window, stateful ? 0 : 1);
+    return check_launch("k_smooth");
+}
+
+// one scenario window of calc_paths: (k_state ->) k_plan -> k_path
+static int paths_window(const LtplLattice* lat, const LtplParams* prm, const LtplDims* w, const LtplBuffers* bf,
+                        cudaStream_t st, bool stateful) {
+    if (stateful) {
+        k_state<<<ctas(w->sub_cnt), kThreads, 0, st>>>(lat->d, *prm, *w, *bf);
+        if (int r = check_launch("k_state")) return r;
+    }
+    if (int r = launch_k_plan(lat, prm, w, bf, st, stateful)) return r;
+    return launch_k_path(lat, prm, w, bf, st, stateful);
+}
+
+// one scenario window of calc_vel_profile.  First tick: k_vel_res (exports its rows itself) (-> k_smooth) (-> k_emergency).
+// Stateful tick: k_ref -> k_vel_res -> k_backup -> k_prefix (-> k_smooth) -> k_export (-> k_emergency)
+static int vel_window(const LtplLattice* lat, const LtplParams* prm, const LtplDims* w, const LtplBuffers* bf,
+                      cudaStream_t st, bool stateful) {
+    const bool smooth = prm->filt_window > 1;
+    if (stateful) {
+        k_ref<<<ctas(w->sub_cnt), kThreads, 0, st>>>(lat->d, *prm, *w, *bf);
+        if (int r = check_launch("k_ref")) return r;
+    }
+    if (int r = launch_k_vel(lat, prm, w, bf, st, stateful)) return r;
+    if (stateful) {
+        k_backup<<<ctas(w->sub_cnt), kThreads, 0, st>>>(*prm, *w, *bf);
+        if (int r = check_launch("k_backup")) return r;
+        k_prefix<<<ctas(LTPL_NSLOT * w->sub_cnt), kThreads, 0, st>>>(*w, *bf);
+        if (int r = check_launch("k_prefix")) return r;
+    }
+    if (smooth)
+        if (int r = launch_smooth(prm, w, bf, st, stateful)) return r;
+    if (stateful)
+        if (int r = launch_export(w, bf, st)) return r;
+    if (prm->incl_emerg_traj) return launch_emergency(prm, w, bf, st);
+    return 0;
+}
+
+enum { kPaths = 1, kVel = 2 };
+
+// The tick protocol: the stages `stages` (calc_paths, calc_vel_profile or both) of a first tick or of a stateful tick.
+// The resets go first, on the caller's stream; then every scenario window runs its whole chain on its stream, one fork /
+// join.  A buffer set with memory (trim != NULL) gets the resets of a session: a first tick exports from point 0 (trim
+// = 0), and a tick without an emergency trajectory leaves em_info at -1, so that the next stateful tick cannot take a
+// stale one for the executed one (k_state).
+static int run_tick(const LtplLattice* lat, const LtplParams* prm, const LtplDims* dm, const LtplBuffers* bf,
+                    void* stream, int stages, bool stateful) {
+    if (int r = validate(lat, prm, dm, bf, stateful)) return r;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const bool paths = stages & kPaths, vel = stages & kVel, memory = bf->trim != nullptr;
+    const size_t B = dm->batch;
+    if (int r = reset_counts(bf, paths, st)) return r;
+    if (memory && paths && !stateful && cudaMemsetAsync(bf->trim, 0, sizeof(int) * 4 * LTPL_NSLOT * B, st) != cudaSuccess)
+        return fail("memset(trim) failed");
+    if (memory && vel && !prm->incl_emerg_traj && bf->em_info &&
+        cudaMemsetAsync(bf->em_info, 0xFF, sizeof(int) * 3 * B, st) != cudaSuccess)
+        return fail("memset(em_info) failed");
+    // `vel` is the start velocity of set_startpos (k_state reads it); the velocity stages of a stateful tick start at the
+    // planned velocity at the cut instead
+    LtplBuffers vbf = *bf;
+    if (stateful) vbf.vel = bf->vel_plan;
+    return for_windows(lat, dm, st, [&](const LtplDims* w, cudaStream_t s) {
+        if (paths)
+            if (int r = paths_window(lat, prm, w, bf, s, stateful)) return r;
+        return vel ? vel_window(lat, prm, w, &vbf, s, stateful) : 0;
+    });
+}
+
+int ltpl_calc_paths_batch(const LtplLattice* lat, const LtplParams* prm, const LtplDims* dm, const LtplBuffers* bf,
+                          void* stream) {
+    return run_tick(lat, prm, dm, bf, stream, kPaths, false);
+}
+
+int ltpl_calc_vel_profile_batch(const LtplLattice* lat, const LtplParams* prm, const LtplDims* dm,
+                                const LtplBuffers* bf, void* stream) {
+    return run_tick(lat, prm, dm, bf, stream, kVel, false);
+}
+
+int ltpl_tick_batch(const LtplLattice* lat, const LtplParams* prm, const LtplDims* dm, const LtplBuffers* bf,
+                    void* stream) {
+    return run_tick(lat, prm, dm, bf, stream, kPaths | kVel, false);
+}
+
+// stateful tick (ltpl_state.cuh):
+//   ltpl_next_calc_paths_batch        k_state -> k_plan<.., true> -> k_path<true>
+//   ltpl_next_calc_vel_profile_batch  k_ref -> k_vel_res<true> -> k_backup -> k_prefix -> k_export
 int ltpl_next_calc_paths_batch(const LtplLattice* lat, const LtplParams* prm, const LtplDims* dm, const LtplBuffers* bf,
                                void* stream) {
-    if (int r = check_stateful(lat, prm, dm, bf)) return r;
-    return launch_paths(lat, prm, dm, bf, static_cast<cudaStream_t>(stream), true);
+    return run_tick(lat, prm, dm, bf, stream, kPaths, true);
 }
 
 int ltpl_next_calc_vel_profile_batch(const LtplLattice* lat, const LtplParams* prm, const LtplDims* dm,
                                      const LtplBuffers* bf, void* stream) {
-    if (int r = check_stateful(lat, prm, dm, bf)) return r;
-    if (bf->vel != bf->vel_plan) return fail("stateful tick: buffers.vel must point at buffers.vel_plan");
-    return launch_vel(lat, prm, dm, bf, static_cast<cudaStream_t>(stream), true);
+    return run_tick(lat, prm, dm, bf, stream, kVel, true);
 }
 
 int ltpl_next_tick_batch(const LtplLattice* lat, const LtplParams* prm, const LtplDims* dm, const LtplBuffers* bf,
                          void* stream) {
-    if (int r = check_stateful(lat, prm, dm, bf)) return r;
-    if (bf->vel != bf->vel_plan) return fail("stateful tick: buffers.vel must point at buffers.vel_plan");
-    return launch_tick(lat, prm, dm, bf, static_cast<cudaStream_t>(stream), true);
+    return run_tick(lat, prm, dm, bf, stream, kPaths | kVel, true);
 }
 
 int ltpl_launch_stage(int stage, const LtplLattice* lat, const LtplParams* prm, const LtplDims* dm,
                       const LtplBuffers* bf, void* stream) {
-    if (int r = check_common(lat, prm, dm, bf)) return r;
+    if (int r = validate(lat, prm, dm, bf, false)) return r;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const LtplDims w = window_dims(dm, 0, 1);   // the whole batch as ONE window: this call times a kernel alone
-    const int nq = LTPL_NSLOT * dm->batch;
     switch (stage) {
         case 0: return ltpl_set_startpos_batch(lat, prm, dm, bf, stream);
-        case 1:
-            if (const char* e = launch_k_plan(lat, prm, &w, bf, st, false)) return fail(e);
-            return check_launch("k_plan");
-        case 2: {
-            size_t smem_path = 0;
-            if (int r = prepare_path_attr(dm, false, &smem_path)) return r;
-            if (cudaMemsetAsync(bf->queue_cnt, 0, kCntInts * sizeof(int), st) != cudaSuccess)
-                return fail("memset(queue_cnt) failed");
-            k_path<false><<<(nq + LTPL_WARPS_PER_CTA - 1) / LTPL_WARPS_PER_CTA, LTPL_WARPS_PER_CTA * 32, smem_path, st>>>(
-                lat->d, *prm, w, *bf);
-            return check_launch("k_path");
-        }
+        case 1: return launch_k_plan(lat, prm, &w, bf, st, false);
+        case 2:
+            if (int r = reset_counts(bf, true, st)) return r;
+            return launch_k_path(lat, prm, &w, bf, st, false);
         case 3:
-            if (cudaMemsetAsync(bf->queue_cnt + 2, 0, sizeof(int), st) != cudaSuccess)
-                return fail("memset(export count) failed");
-            if (launch_k_vel(lat, prm, &w, bf, st) != cudaSuccess) return fail(kVelCapacity);
-            return check_launch("k_vel");
-        case 4:
-            k_export<<<(nq + LTPL_WARPS_PER_CTA_EXPORT - 1) / LTPL_WARPS_PER_CTA_EXPORT,
-                       LTPL_WARPS_PER_CTA_EXPORT * 32, 0, st>>>(w, *bf);
-            return check_launch("k_export");
+            if (int r = reset_counts(bf, false, st)) return r;
+            return launch_k_vel(lat, prm, &w, bf, st, false);
+        case 4: return launch_export(&w, bf, st);
         default: return fail("ltpl_launch_stage: unknown stage");
     }
 }

@@ -90,6 +90,8 @@ struct LtplLattice {
     int n_sub = 1, sub_min = LTPL_SUB_MIN;
     cudaStream_t aux[LTPL_MAX_SUB - 1] = {};
     cudaEvent_t ev_fork = nullptr, ev_join[LTPL_MAX_SUB - 1] = {};
+    // dynamic shared memory each kernel family (ltpl_api.cu: SmemFamily) may use on this handle's device
+    mutable size_t smem_allowed[4] = {};
 };
 
 // scenario of a one-warp-per-scenario kernel inside the launch's sub-batch window (-1: none)

@@ -431,7 +431,7 @@ k_backup(const __grid_constant__ LtplParams prm, const __grid_constant__ LtplDim
         const double dmq = prm.drag_coeff / prm.m_veh, inv_ay = 1.0 / prm.gg_ay;
         // location dependent local_gg of the LAST tick along the backup path (__backup_path_gg, OTH:970-975), raw
         const double* ggr = bf.prev_gg ? bf.prev_gg + (size_t)q * dm.p_max + m_b + cut + pref : nullptr;
-        double v0 = bf.vel[b];                                  // == vel_plan (the host points `vel` at it)
+        double v0 = bf.vel[b];                                  // == vel_plan (run_tick launches k_backup so)
         if (v0 < 0.0) v0 = 0.0;
         double w = v0 * v0, s = 0.0;
         bool stopped = false;

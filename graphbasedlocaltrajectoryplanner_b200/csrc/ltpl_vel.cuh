@@ -28,6 +28,8 @@ __device__ __forceinline__ double acc_brake(double w, double kabs, double ax_max
     return fma(-w, dm, -acc_tire(w, kabs, ax_max, inv_ay, exp_));
 }
 
+#define LTPL_WARPS_PER_CTA_EXPORT 8
+
 // (P, 7) rows s, x, y, psi, kappa, vx, ax of every kept trajectory, cut to nmbr_export_points (OTH:941, LTPL:401-406)
 __global__ void __launch_bounds__(LTPL_WARPS_PER_CTA_EXPORT * 32)
 k_export(const __grid_constant__ LtplDims dm, const __grid_constant__ LtplBuffers bf) {

@@ -387,7 +387,7 @@ __device__ __forceinline__ void vr_convert_el(float* X0, float* X4, double* s_ou
 }
 
 // STATE: stateful tick (ltpl_state.cuh) -- every path starts at its cut index + the vel_course rows (bf.trim), the planned
-// velocity comes from bf.vel (pointed at vel_plan by the host), the follow-mode object distance from bf.obj_dist (k_ref)
+// velocity comes from bf.vel (= vel_plan in the library's launch), the follow-mode object distance from bf.obj_dist (k_ref)
 // EXP1: friction-ellipse exponent 1.0 (LTPL:190 default): no pow on the chain
 //
 // Every device function with a long body has ONE call site (the sweeps are out of line on top): the rounds of the three

@@ -484,38 +484,28 @@ class BatchPlanner(object):
             yield self.h_out_sets[j]
 
     # -- kernels ---------------------------------------------------------------------------------------------------------------
-    def _call(self, fn, what):
-        capi.check(self.lib, fn(self.handle, C.byref(self.params), C.byref(self.dims), C.byref(self.buf), self.stream),
-                   what)
+    def _call(self, name):
+        capi.check(self.lib, getattr(self.lib, name)(self.handle, C.byref(self.params), C.byref(self.dims),
+                                                     C.byref(self.buf), self.stream), name)
+
+    def _call_vel(self, name):
+        """a call that includes calc_vel_profile: its trajectories get the next ids (+10 per call, OTH:669)"""
+        self._tick_count += 1
+        self.params.traj_base_id = 10 * self._tick_count
+        self._call(name)
 
     def set_startpos(self) -> None:
-        if self._state is not None:
-            self._state["zone_s0"].fill_(-1)   # zones are processed anew by the first tick (GLNT:43-77)
-        self._call(self.lib.ltpl_set_startpos_batch, "ltpl_set_startpos_batch")
+        self._call("ltpl_set_startpos_batch")
 
     def calc_paths(self) -> None:
-        if self._state is not None:
-            self.t["trim"].zero_()   # a first tick exports from point 0
-        self._call(self.lib.ltpl_calc_paths_batch, "ltpl_calc_paths_batch")
-
-    def _no_stale_emergency(self) -> None:
-        if self._state is not None and not self.params.incl_emerg_traj:
-            self.t["em_info"].fill_(-1)   # a later stateful tick must not take an older emergency trajectory for executed
+        self._call("ltpl_calc_paths_batch")
 
     def calc_vel_profile(self) -> None:
-        self._no_stale_emergency()
-        self._tick_count += 1
-        self.params.traj_base_id = 10 * self._tick_count   # OTH:669
-        self._call(self.lib.ltpl_calc_vel_profile_batch, "ltpl_calc_vel_profile_batch")
+        self._call_vel("ltpl_calc_vel_profile_batch")
 
     def tick(self) -> None:
         """calc_paths + calc_vel_profile back to back."""
-        if self._state is not None:
-            self.t["trim"].zero_()   # a first tick exports from point 0
-        self._no_stale_emergency()
-        self._tick_count += 1
-        self.params.traj_base_id = 10 * self._tick_count
-        self._call(self.lib.ltpl_tick_batch, "ltpl_tick_batch")
+        self._call_vel("ltpl_tick_batch")
 
     # -- stateful tick (DESIGN.md section 11, csrc/ltpl_state.cuh) ----------------------------------------------
     _BIG = ("path", "node_idx", "nodes", "coeff", "s_vx_ax", "em_vx")            # swapped by pointer
@@ -539,16 +529,9 @@ class BatchPlanner(object):
         self.buf.trim = t["trim"].data_ptr()
         self._state = st
 
-    def next_calc_paths(self, sc: ScenarioBatch, sel_action, t_const, vel_est=None) -> None:
-        """calc_paths of a stateful tick (OTH:289-516 with the iterative memory): ``sc`` carries the object
-        lists (its poses are only used by ``next_calc_vel_profile``), ``sel_action`` = action id (capi.ACT_*) every
-        scenario executed since the last tick, ``t_const`` = min(average calculation time * calc_time_safety, 0.5) per
-        scenario (OTH:353-375; the caller keeps the moving average).  The previous tick (tick() / calc_paths() +
-        calc_vel_profile() after set_startpos(), or a stateful tick) must have run on this planner.
-
-        Host side of one call: pointer swaps, the host memcpy into the pinned staging set, ONE packed H2D copy (scenario
-        arrays incl. sel_action / t_const), ONE device copy (the small per-path arrays of the last tick) and the
-        library call."""
+    def _stage_next(self, sc: ScenarioBatch, sel_action, t_const, vel_est) -> None:
+        """host side of a stateful tick: pointer swaps, the host memcpy into the pinned staging set, ONE packed H2D copy
+        (scenario arrays incl. sel_action / t_const) and ONE device copy (the small per-path arrays of the last tick)."""
         if sc.size != self.dims.batch:
             raise ValueError("stateful tick: the batch size must not change within a session (re-anchor with "
                              "set_startpos on a new batch)")
@@ -595,27 +578,27 @@ class BatchPlanner(object):
         if self.on_device_start is not None:   # measurement hook: the host staging ends here, the device work begins
             self.on_device_start()
         self.upload()
-        self._call(self.lib.ltpl_next_calc_paths_batch, "ltpl_next_calc_paths_batch")
+
+    def next_calc_paths(self, sc: ScenarioBatch, sel_action, t_const, vel_est=None) -> None:
+        """calc_paths of a stateful tick (OTH:289-516 with the iterative memory): ``sc`` carries the object
+        lists (its poses are only used by ``next_calc_vel_profile``), ``sel_action`` = action id (capi.ACT_*) every
+        scenario executed since the last tick, ``t_const`` = min(average calculation time * calc_time_safety, 0.5) per
+        scenario (OTH:353-375; the caller keeps the moving average).  The previous tick (tick() / calc_paths() +
+        calc_vel_profile() after set_startpos(), or a stateful tick) must have run on this planner."""
+        self._stage_next(sc, sel_action, t_const, vel_est)
+        self._call("ltpl_next_calc_paths_batch")
 
     def next_calc_vel_profile(self, pos_est=None, vel_est=None) -> None:
         """calc_vel_profile of a stateful tick (OTH:518-601 + 603-1040): position / velocity estimates per
         scenario (None: the poses / velocities staged by ``next_calc_paths``)."""
-        buf, st = self.buf, self._state
         if pos_est is not None or vel_est is not None:
             self.set_estimates(pos_est, vel_est)
-        keep_vel = buf.vel
-        buf.vel = st["vel_plan"].data_ptr()                   # the planned velocity at the cut replaces the start velocity
-        try:
-            self._tick_count += 1
-            self.params.traj_base_id = 10 * self._tick_count
-            self._call(self.lib.ltpl_next_calc_vel_profile_batch, "ltpl_next_calc_vel_profile_batch")
-        finally:
-            buf.vel = keep_vel
+        self._call_vel("ltpl_next_calc_vel_profile_batch")
 
     def next_tick(self, sc: ScenarioBatch, sel_action, t_const, vel_est=None) -> None:
-        """One stateful tick for the whole batch: ``sc.pos`` = position estimates."""
-        self.next_calc_paths(sc, sel_action, t_const, vel_est=vel_est)   # vel_est travels in the packed upload
-        self.next_calc_vel_profile()
+        """One stateful tick for the whole batch in one library call: ``sc.pos`` = position estimates."""
+        self._stage_next(sc, sel_action, t_const, vel_est)   # vel_est travels in the packed upload
+        self._call_vel("ltpl_next_tick_batch")
 
     def launch_count(self) -> int:
         return int(self.lib.ltpl_launch_count())

@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define LTPL_ABI_VERSION 13
+#define LTPL_ABI_VERSION 14
 
 /* action ids (OTH:14-17 ACTION_ID_MAP) */
 #define LTPL_ACT_NONE (-1)
@@ -187,7 +187,8 @@ typedef struct LtplBuffers {
     /* scenario inputs (Graph_LTPL.set_startpos / calc_paths arguments)                                                 */
     const double* pos;        /* [B][2]                                                                                  */
     const double* heading;    /* [B]                                                                                     */
-    const double* vel;        /* [B]  start velocity of set_startpos (planned velocity of the first tick, OTH:595)       */
+    const double* vel;        /* [B]  start velocity of set_startpos (planned velocity of the first tick, OTH:595);      */
+                              /*      in every tick, stateful ones included (k_state restarts from it, OTH:597)          */
     const double* vel_est;    /* [B]  velocity estimate passed to calc_vel_profile (follow-mode controller, OTH:794)     */
     const int32_t* n_obj;     /* [B]                                                                                     */
     const double* obj;        /* [B][K][5] X, Y, theta, v, length (OLI:96-141)                                           */
@@ -238,6 +239,12 @@ typedef struct LtplBuffers {
     /* ---- stateful tick (ltpl_next_*_batch, see DESIGN.md section 11): the iterative memory of            */
     /* OnlineTrajectoryHandler (OTH:64-87) = the output buffers of the previous tick (a second buffer set, used            */
     /* ping-pong) + per-path trims instead of the slicing of OTH:705-731.  NULL for first ticks.                           */
+    /* A buffer set carries memory exactly when `trim` is non-NULL.  The library then keeps the memory consistent itself: */
+    /*   - ltpl_set_startpos_batch sets zone_s0 (if non-NULL) to -1: the first tick processes the zones anew;            */
+    /*   - a first tick (ltpl_calc_paths_batch, ltpl_tick_batch) sets trim to 0: it exports from point 0;                */
+    /*   - the velocity part of any tick without params.incl_emerg_traj sets em_info (if non-NULL) to -1, so that the   */
+    /*     next stateful tick cannot take a stale emergency trajectory for the executed one.                              */
+    /* With trim == NULL (a stateless planner) none of these resets runs.                                                 */
     const double* prev_path;        /* previous tick's `path`                                                             */
     const int32_t* prev_path_len;   /* ... `path_len`                                                                     */
     const int32_t* prev_node_idx;   /* ... `node_idx`                                                                     */
@@ -255,13 +262,13 @@ typedef struct LtplBuffers {
     int32_t* st_info;               /* [B][8] k_state: prev path id, prev m, prev L, constant nodes, #factored edges, e0..e2 */
     int32_t* trim;                  /* [NSLOT*B][4] m = first memory point, L = first memory node, c = first trajectory   */
                                     /*     point (path-plane indices of THIS tick, OTH:586-598, 705-731), pref = #points    */
-                                    /*     of vel_course; zero on first ticks                                               */
-    double* vel_plan;               /* [B] planned velocity at the cut (OTH:572); the kernels read it through `vel`        */
+                                    /*     of vel_course; set to zero by a first tick                                       */
+    double* vel_plan;               /* [B] planned velocity at the cut (OTH:572): the start of the velocity profiles      */
     double* course;                 /* [B][n_export] vel_course (OTH:574): at most the rows of an exported trajectory      */
     double* obj_dist;               /* [B] s_obj - s_start on the cut follow path (OTH:774-784)                            */
     int32_t* zone_s0;               /* [B] start layer of the tick in which the scenario's zone was processed (GLNT:43-77:  */
-                                    /*     the unblock window is evaluated once), -1: not yet; needed for zones in stateful  */
-                                    /*     ticks, optional (NULL) otherwise                                                   */
+                                    /*     the unblock window is evaluated once), -1: not yet (set by set_startpos); needed  */
+                                    /*     for zones in stateful ticks, optional (NULL) otherwise                             */
     /* executed 'emergency' trajectory (sel_action = LTPL_ACT_EMERGENCY): get_ref_idx (OTH:518-601) reads the velocity of  */
     /* THAT trajectory; optional (NULL: such scenarios are flagged LTPL_SC_STATE_FALLBACK)                                 */
     double* em_vx;                  /* [B][n_export] f64 velocity of this tick's emergency trajectory (k_emergency)        */

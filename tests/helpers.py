@@ -172,6 +172,23 @@ def zone_of(g, b, tick=0):
                             np.zeros((2, 2))]}
 
 
+def tick_snapshot(pl):
+    """the results of a BatchPlanner's last tick as arrays that are byte-comparable across runs: rows of the compact
+    export are gathered through traj_row (their order is unspecified), entries behind the valid lengths are cleared."""
+    f = pl.fetch("action_id", "status", "n_nodes", "nodes", "path_len", "traj_len", "traj_row", "traj", "em_info",
+                 "sc_flags")
+    ok = f["traj_row"] >= 0
+    rows = np.zeros(f["traj_row"].shape + f["traj"].shape[1:], dtype=np.float32)
+    rows[ok] = f["traj"][f["traj_row"][ok]]
+    rows[np.arange(rows.shape[2])[None, None, :] >= f["traj_len"][..., None]] = 0.0
+    nodes = f["nodes"].copy()
+    nodes[np.arange(nodes.shape[2])[None, None, :] >= f["n_nodes"][..., None]] = -1
+    em = f["em_info"].copy()
+    em_rows = f["traj"][np.maximum(em[:, 0], 0)] * (em[:, 0] >= 0)[:, None, None]
+    return dict(action_id=f["action_id"], status=f["status"], nodes=nodes, path_len=f["path_len"],
+                traj_len=f["traj_len"], rows=rows, em_len=em[:, 1], em_rows=em_rows, flags=f["sc_flags"])
+
+
 def compare_emergency(rec, g, b, ctx=""):
     """'emergency' entry (OTH:1027-1034) of a tick record against the zone / emergency fixture."""
     n = int(g["em_len"][b])

@@ -173,24 +173,8 @@ def test_tick_under_cuda_graph_capture_replays_identically():
     pl.stage_scenarios(sc)
     pl.upload()
     pl.set_startpos()
-    names = ("action_id", "status", "n_nodes", "nodes", "path_len", "traj_len", "traj_row", "traj", "em_info", "sc_flags")
-
-    def snapshot():
-        torch.cuda.synchronize()
-        f = pl.fetch(*names)
-        ok = f["traj_row"] >= 0
-        rows = np.zeros(f["traj_row"].shape + f["traj"].shape[1:], dtype=np.float32)
-        rows[ok] = f["traj"][f["traj_row"][ok]]
-        rows[np.arange(rows.shape[2])[None, None, :] >= f["traj_len"][..., None]] = 0.0
-        nodes = f["nodes"].copy()
-        nodes[np.arange(nodes.shape[2])[None, None, :] >= f["n_nodes"][..., None]] = -1
-        em = f["em_info"].copy()
-        em_rows = f["traj"][np.maximum(em[:, 0], 0)] * (em[:, 0] >= 0)[:, None, None]
-        return dict(action_id=f["action_id"], status=f["status"], nodes=nodes, path_len=f["path_len"],
-                    traj_len=f["traj_len"], rows=rows, em_len=em[:, 1], em_rows=em_rows, flags=f["sc_flags"])
-
     pl.tick()                                   # eager (also the warm-up that sets the kernels' attributes)
-    want = snapshot()
+    want = H.tick_snapshot(pl)
     assert (want["traj_len"] > 0).sum() > 300
     side = torch.cuda.Stream()
     side.wait_stream(torch.cuda.current_stream())
@@ -201,6 +185,43 @@ def test_tick_under_cuda_graph_capture_replays_identically():
     for name in ("traj", "traj_row", "traj_len", "action_id", "status"):   # the replay has to produce everything again
         pl.t[name].zero_()
     graph.replay()
-    got = snapshot()
+    got = H.tick_snapshot(pl)
     for k in want:
         assert np.array_equal(got[k], want[k]), k
+
+
+@pytest.mark.parametrize("dev_b", ["cuda:0", "cuda:1"])
+def test_planners_sharing_the_shared_memory_attribute(dev_b):
+    """the dynamic shared-memory limit of a kernel belongs to the device and is shared by every planner on it.  On the
+    open lattice the velocity kernel needs more than the 48 KB default: 55 KB, and 77 KB with local_gg planes.  Planner
+    A (local_gg planes, cuda:0) plans a tick, then planner B (no planes) in the same thread on the same GPU or on a second
+    one, then A again: every tick runs, and A's two ticks are identical."""
+    import torch
+    if torch.cuda.device_count() <= torch.device(dev_b).index:
+        pytest.skip("needs two GPUs")
+    from graphbasedlocaltrajectoryplanner_b200.planner import BatchPlanner
+    from graphbasedlocaltrajectoryplanner_b200.scenarios import Track, make_scenarios
+    g = H.golden("ticks_default.npz")
+    trk = Track(H.track_csv_for("open"))
+    sc = make_scenarios(trk, 64, seed=79, n_obj_min=0, n_obj_max=3, s_max=trk.length - 10.0)
+
+    def tick(pl, local_gg):
+        with torch.cuda.device(pl.device):
+            pl.stage_scenarios(sc)
+            pl.upload()
+            pl.set_startpos()
+            pl.calc_paths()
+            if local_gg:
+                pl.set_local_gg_planes(*H.local_gg_planes(pl))
+            pl.calc_vel_profile()
+            return H.tick_snapshot(pl)
+
+    a, b = BatchPlanner(H.lattice_for("open"), device="cuda:0"), BatchPlanner(H.lattice_for("open"), device=dev_b)
+    for pl in (a, b):
+        pl.set_vel_params(ax_max_machines=g["ax_max_machines"], **VEL)
+    first = tick(a, True)
+    assert (tick(b, False)["traj_len"] > 0).sum() > 64
+    again = tick(a, True)
+    assert (first["traj_len"] > 0).sum() > 64
+    for k in first:
+        assert np.array_equal(again[k], first[k]), k
