@@ -12,7 +12,7 @@ import os
 import subprocess
 import sys
 
-ABI_VERSION = 14
+ABI_VERSION = 15
 MAX_SUB = 8
 NSLOT = 3
 KMAX = 16

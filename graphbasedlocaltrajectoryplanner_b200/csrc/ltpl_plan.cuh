@@ -4,7 +4,7 @@
 #include "ltpl_common.cuh"
 
 #define LTPL_KMAX 16          // object slots per scenario held in shared memory
-#define LTPL_DMAX 32          // obstacle discs per scenario (one warp ballot): on-track vehicles + their prediction points
+#define LTPL_DMAX 32          // obstacle discs per chunk of the disc stage (one warp ballot; a scenario may hold any number)
 #define LTPL_WARPS_PER_CTA 4
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -442,11 +442,14 @@ __device__ __forceinline__ int dp_goal(const LatDev& lt, int lane, const DpCtx& 
 // ---------------------------------------------------------------------------------------------------------------------
 struct PlanSmem {  // per warp, followed by dist / mask / pred (sizes depend on the lattice)
     double vx[LTPL_KMAX], vy[LTPL_KMAX], vr[LTPL_KMAX], vv[LTPL_KMAX];
-    // obstacle discs (GLNT:169-189): per on-track vehicle its current position followed by its prediction points
+    double vref[LTPL_KMAX];               // inflated disc radius, squared (GB:626-629)
+    double vpx[LTPL_KMAX], vpy[LTPL_KMAX]; // built-in 0.2 s prediction point of a vehicle without a 'prediction' array
+    // obstacle discs (GLNT:169-189): per on-track vehicle its current position followed by its prediction points; the
+    // discs of a scenario are numbered in that order and visited in chunks of 32, disc c0 + l of a chunk at index l
     double dx[LTPL_DMAX], dy[LTPL_DMAX], dref[LTPL_DMAX];
     int vd0[LTPL_KMAX], vdn[LTPL_KMAX];   // first disc of a vehicle, number of prediction discs behind it
-    int n_veh;
-    int pad[3];
+    int vslot[LTPL_KMAX];                 // object slot of the vehicle's obj_pred row, -1: built-in 0.2 s point
+    int vlayer[LTPL_KMAX];                // layer of the vehicle's last disc (-1: outside the planning range), q14
 };
 
 // per warp: PlanSmem | dist f64[2 maxn] | dsave f64[maxn] | meta int4[hl] | mask u32[mask_words] | pred u8[hl maxn]
@@ -523,6 +526,50 @@ __device__ __forceinline__ int disc_pairs(const LatDev& lt, int o, int p_start, 
     return o;
 }
 
+// One chunk of k_plan's disc stage (discs c0 .. c0 + 31 of the scenario): lane l materialises disc d = c0 + l into
+// ps->dx / dy / dref[l] and returns the layer pairs it can block, (pa + 1) | (pb + 1) << 16 (disc_pairs, 0: none); the
+// layer of every vehicle whose last disc lies in the chunk goes to ps->vlayer (q14).  Out of line: the warp-wide
+// fallback of lanes_closest_point is a call, and inside k_plan's chunk loop every value live across it would take a
+// spill slot.
+__device__ __noinline__ int chunk_discs(const LatDev& lt, const LtplDims& dm, const LtplBuffers& bf, PlanSmem* ps,
+                                        int b, int c0, int n_disc, int n_veh, int start_layer, int end_layer, int lane) {
+    const int d = c0 + lane;
+    const bool act = d < n_disc;
+    double ox = 0.0, oy = 0.0;
+    if (act) {
+        // vehicle of disc d: the last one whose first disc is <= d; position j = 0, then its prediction points
+        int v = 0;
+        #pragma unroll 1
+        for (int w = 1; w < n_veh; ++w)
+            if (ps->vd0[w] <= d) v = w;
+        const int j = d - ps->vd0[v], slot = ps->vslot[v];
+        if (j == 0) {
+            ox = ps->vx[v];
+            oy = ps->vy[v];
+        } else if (slot < 0) {
+            ox = ps->vpx[v];
+            oy = ps->vpy[v];
+        } else {
+            const double* pp = bf.obj_pred + (((size_t)b * dm.k_obj + slot) * dm.k_pred + (j - 1)) * 2;
+            ox = pp[0];
+            oy = pp[1];
+        }
+        ps->dx[lane] = ox;
+        ps->dy[lane] = oy;
+        ps->dref[lane] = ps->vref[v];
+    }
+    const int o = lanes_closest_point(lt, lt.grid_refline, lt.refline, lt.L, ox, oy, act, lane);
+    int pa = -1, pb = -1;
+    if (act) {
+        const int layer = disc_pairs(lt, o, start_layer, end_layer, &pa, &pb);
+        // current position, then the prediction points: the LAST one sets obj_layer (q14)
+        #pragma unroll 1
+        for (int w = 0; w < n_veh; ++w)
+            if (ps->vd0[w] + ps->vdn[w] == d) ps->vlayer[w] = layer;
+    }
+    return (pa + 1) | ((pb + 1) << 16);
+}
+
 // action-set table of k_plan packed into one integer: action a holds its name (LTPL_ACT_STRAIGHT .. LTPL_ACT_RIGHT) in
 // bits 5a .. 5a+2 and its filter in bits 5a+3 .. 5a+4
 __device__ __forceinline__ int act_entry(int a, int name, int filter) { return (name | filter << 3) << (5 * a); }
@@ -573,17 +620,9 @@ k_plan(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm
     if (bf.sc_flags[b] != 0) return;
     LTPL_PH_INIT
 
-    const int start_layer = bf.start_node[2 * b], start_node = bf.start_node[2 * b + 1];
-    const int p0 = bf.const_len[b];
-    size_t cplane = (size_t)B * dm.p0_max;
-    const double* cs = bf.const_seg + (size_t)b * dm.p0_max;
-    int cnd = 1;   // entries of the node / node-index / coefficient lists in front of the start node
-    if (STATE) {
-        const int* sinfo = bf.st_info + 8 * (size_t)b;
-        cplane = (size_t)LTPL_NSLOT * B * dm.p_max;
-        cs = bf.prev_path + (size_t)sinfo[0] * dm.p_max + sinfo[1];
-        cnd = sinfo[3];
-    }
+    const int start_layer = bf.start_node[2 * b];
+    // entries of the node / node-index / coefficient lists in front of the start node
+    const int cnd = STATE ? bf.st_info[8 * (size_t)b + 3] : 1;
 
     // ---- OLI.process_object_list (OLI:96-141): drop off-track objects, radius = length / 2, prediction points: the
     // caller's 'prediction' array (OLI:117-119) or one constant-velocity point at 0.2 s (OLI:121-127) ----
@@ -611,36 +650,21 @@ k_plan(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm
         }
         n_disc = __shfl_sync(LTPL_FULL, incl, 31);
         n_veh = __popc(in_mask);
-        if (n_disc > LTPL_DMAX) {   // (the reference has no limit; one warp ballot holds 32 discs)
-            if (lane == 0) bf.sc_flags[b] = LTPL_SC_CAPACITY;
-            return;
-        }
         if (inside) {
-            const int v_i = __popc(in_mask & ((1u << lane) - 1u)), d_i = incl - mine;
+            const int v_i = __popc(in_mask & ((1u << lane) - 1u));
             const double th = o[2], v = o[3], r = o[4] / 2.0;
             ps->vx[v_i] = ox;
             ps->vy[v_i] = oy;
             ps->vr[v_i] = r;
             ps->vv[v_i] = v;
-            ps->vd0[v_i] = d_i;
+            ps->vd0[v_i] = incl - mine;
             ps->vdn[v_i] = n_pd;
+            ps->vslot[v_i] = (np_k < 0) ? -1 : lane;
             // obstacle_ref = (r + veh_width / 2)^2 + stepsize^2 / 4  (GB:626-629)
-            const double ref = __dadd_rn(sq_rn(__dadd_rn(r, __ddiv_rn(lt.veh_width, 2.0))),
-                                         __ddiv_rn(sq_rn(lt.step), 4.0));
-            ps->dx[d_i] = ox;
-            ps->dy[d_i] = oy;
-            ps->dref[d_i] = ref;
+            ps->vref[v_i] = __dadd_rn(sq_rn(__dadd_rn(r, __ddiv_rn(lt.veh_width, 2.0))), __ddiv_rn(sq_rn(lt.step), 4.0));
             if (np_k < 0) {
-                ps->dx[d_i + 1] = __dsub_rn(ox, __dmul_rn(__dmul_rn(sin(th), v), 0.2));
-                ps->dy[d_i + 1] = __dadd_rn(oy, __dmul_rn(__dmul_rn(cos(th), v), 0.2));
-                ps->dref[d_i + 1] = ref;
-            } else {
-                const double* pp = bf.obj_pred + (((size_t)b * dm.k_obj + lane) * dm.k_pred) * 2;
-                for (int j = 0; j < np_k; ++j) {
-                    ps->dx[d_i + 1 + j] = pp[2 * j];
-                    ps->dy[d_i + 1 + j] = pp[2 * j + 1];
-                    ps->dref[d_i + 1 + j] = ref;
-                }
+                ps->vpx[v_i] = __dsub_rn(ox, __dmul_rn(__dmul_rn(sin(th), v), 0.2));
+                ps->vpy[v_i] = __dadd_rn(oy, __dmul_rn(__dmul_rn(cos(th), v), 0.2));
             }
         }
     }
@@ -662,19 +686,28 @@ k_plan(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm
 
     // ---- obstacles -> blocked edges, closest object (GLNT:165-213) ----
     int closest_dist = -1, closest_idx = -1, con_layer = -1, con_node = -1;
-    int my_pa = -1, my_pb = -1;  // lane d: layer pairs disc d can block
-    int my_layer = -1;           // lane d: nearest reference-line layer of disc d, -1 outside the planning range
     __syncwarp();
-    {
-        const bool act = lane < n_disc;
-        const double ox = act ? ps->dx[lane] : 0.0, oy = act ? ps->dy[lane] : 0.0;
-        const int o = lanes_closest_point(lt, lt.grid_refline, lt.refline, lt.L, ox, oy, act, lane);
-        if (act) my_layer = disc_pairs(lt, o, start_layer, end_layer, &my_pa, &my_pb);
+    #pragma unroll 1
+    for (int c0 = 0; c0 < n_disc; c0 += LTPL_DMAX) {
+        const int pr = chunk_discs(lt, dm, bf, ps, b, c0, n_disc, n_veh, start_layer, end_layer, lane);  // lane l: disc c0 + l
+        __syncwarp();
+        #pragma unroll 1
+        for (int dl = 0; dl < LTPL_DMAX && c0 + dl < n_disc; ++dl) {  // one sweep per distinct layer pair of the chunk
+            const int pd = __shfl_sync(LTPL_FULL, pr, dl);
+            #pragma unroll 1
+            for (int slot = 0; slot < 2; ++slot) {
+                const int a = (slot ? (pd >> 16) : (pd & 0xffff)) - 1;
+                if (a < 0) continue;
+                const unsigned discs = __ballot_sync(LTPL_FULL, (pr & 0xffff) == a + 1 || (pr >> 16) == a + 1);
+                if (discs & ((1u << dl) - 1u)) continue;  // swept together with an earlier disc of the chunk
+                block_pair(lt, lane, a, discs, ps, mask, e_base);
+            }
+        }
+        __syncwarp();
     }
     #pragma unroll 1
     for (int v = 0; v < n_veh; ++v) {
-        // current position, then the prediction points: the LAST one sets obj_layer (q14)
-        const int obj_layer = __shfl_sync(LTPL_FULL, my_layer, ps->vd0[v] + ps->vdn[v]);
+        const int obj_layer = ps->vlayer[v];
         if (obj_layer >= 0) {
             int ld = obj_layer - start_layer;
             if (ld < 0) ld = lt.L - start_layer + obj_layer;
@@ -685,19 +718,6 @@ k_plan(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm
             }
         }
     }
-    __syncwarp();
-    #pragma unroll 1
-    for (int d = 0; d < n_disc; ++d) {  // one sweep per distinct layer pair, shared by every disc that touches it
-        #pragma unroll 1
-        for (int slot = 0; slot < 2; ++slot) {
-            const int a = __shfl_sync(LTPL_FULL, slot ? my_pb : my_pa, d);
-            if (a < 0) continue;
-            const unsigned discs = __ballot_sync(LTPL_FULL, my_pa == a || my_pb == a);
-            if (discs & ((1u << d) - 1u)) continue;  // swept together with an earlier disc
-            block_pair(lt, lane, a, discs, ps, mask, e_base);
-        }
-    }
-    __syncwarp();
     if (closest_dist >= 0) {  // GLNT:206-213
         const int nb = lt.node_off[con_layer];
         const ArgMinD m = warp_closest_point(lt.node_xy + nb, lt.node_off[con_layer + 1] - nb, ps->vx[closest_idx],
@@ -707,6 +727,16 @@ k_plan(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm
     LTPL_PH(18)
 
     // ---- objects in / beside the constant path segment (MOPG:76-122) ----
+    // (read here: nothing of the constant segment stays live across the disc stage)
+    const int start_node = bf.start_node[2 * b + 1];
+    const int p0 = bf.const_len[b];
+    size_t cplane = (size_t)B * dm.p0_max;
+    const double* cs = bf.const_seg + (size_t)b * dm.p0_max;
+    if (STATE) {
+        const int* sinfo = bf.st_info + 8 * (size_t)b;
+        cplane = (size_t)LTPL_NSLOT * B * dm.p_max;
+        cs = bf.prev_path + (size_t)sinfo[0] * dm.p_max + sinfo[1];
+    }
     bool obj_in_const = false, obj_beside = false;
     if (p0 >= 2) {
         // MOPG:80-84: pos_est of the previous calc_vel_profile call; None on the first tick -> first point of the segment
@@ -992,7 +1022,7 @@ k_plan(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm
     if (lane == 0) {
         bool any = false;
         for (int s = 0; s < LTPL_NSLOT; ++s) any |= (bf.action_id[s * B + b] != LTPL_ACT_NONE);
-        if (!any && p0 > 2) {
+        if (!any && bf.const_len[b] > 2) {   // (re-read: p0 is not kept live across the searches)
             const int q = b;
             int* nd = bf.nodes + (size_t)q * dm.h_max * 2;
             if (STATE) {

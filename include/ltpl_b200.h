@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define LTPL_ABI_VERSION 14
+#define LTPL_ABI_VERSION 15
 
 /* action ids (OTH:14-17 ACTION_ID_MAP) */
 #define LTPL_ACT_NONE (-1)
@@ -234,8 +234,8 @@ typedef struct LtplBuffers {
     /* explicit prediction arrays of the objects (object dict key 'prediction', OLI:117-119); may be NULL when k_pred == 0 */
     const double* obj_pred;   /* [B][K][k_pred][2] x, y                                                                  */
     const int32_t* n_pred;    /* [B][K] number of prediction points of the object, -1: none given -> one constant-        */
-                              /*        velocity point at 0.2 s (OLI:121-127).  At most 32 discs (on-track objects +     */
-                              /*        their prediction points) per scenario, else LTPL_SC_CAPACITY                     */
+                              /*        velocity point at 0.2 s (OLI:121-127).  Any number of points, at most k_pred    */
+                              /*        are read; every point is one obstacle disc, with no limit per scenario          */
     /* ---- stateful tick (ltpl_next_*_batch, see DESIGN.md section 11): the iterative memory of            */
     /* OnlineTrajectoryHandler (OTH:64-87) = the output buffers of the previous tick (a second buffer set, used            */
     /* ping-pong) + per-path trims instead of the slicing of OTH:705-731.  NULL for first ticks.                           */

@@ -2,6 +2,7 @@
 Run as  compute-sanitizer --tool memcheck|racecheck|initcheck|synccheck python tools/gpu_sanitize.py"""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import numpy as np
 from tests import helpers as H
 from graphbasedlocaltrajectoryplanner_b200.planner import BatchPlanner
@@ -28,6 +29,17 @@ sel = ps.t["action_id"].max(dim=0).values.clamp(min=0).cpu().numpy()   # an acti
 ps.next_tick(sc, sel_action=sel, t_const=0.1)
 r = ps.records()
 print("smoothed stateful tick, trajectories:", sum(len(x.get("traj", {})) for x in r))
-mb = make_velocity_microbench(200, 150, seed=3)
+# long prediction arrays (k_plan's disc stage in chunks of 32): 3 objects x 40 points = 123 discs per scenario, a first
+# tick and a stateful tick
+from bench_pred import with_predictions  # noqa: E402
+sc = with_predictions(make_scenarios(Track(H.TRACK_CSV), n, seed=79, n_obj_min=3, n_obj_max=3), 40)
+pp = BatchPlanner(H.lattice_for("default"), device="cuda:0", stateful=True)
+pp.set_vel_params(ax_max_machines=g["ax_max_machines"], **VEL)
+pp.stage_scenarios(sc); pp.upload(); pp.set_startpos(); pp.tick()
+sel = pp.t["action_id"].max(dim=0).values.clamp(min=0).cpu().numpy()
+pp.next_tick(sc, sel_action=sel, t_const=0.1)
+r = pp.records()
+print("long-prediction stateful tick, trajectories:", sum(len(x.get("traj", {})) for x in r))
+mb =make_velocity_microbench(200, 150, seed=3)
 vx, ax = calc_vel_profile_batch(pl, mb["kappa"], mb["el"], mb["v_start"], mb["v_end"])
 print("dense vx mean", float(np.mean(vx)))
