@@ -44,6 +44,12 @@ REQ_PATH_DICT_ENTRIES = ['globtraj_input_path', 'graph_store_path', 'ltpl_offlin
                          'graph_log_id', 'log_path']
 
 
+def physical_objects(object_list) -> list:
+    """the entries the object filter sees (OLI:104-112): 'physical' ones, in list order, on the track or not (the track
+    test runs on the device); their number is bounded by BatchPlanner.max_objects, not by the on-track count."""
+    return [o for o in (object_list or []) if o.get('type') == 'physical']
+
+
 class ActionSetView(object):
     """Lazy sequence over the scenarios of a batched result (Graph_LTPL.unpack_batch): ``view[b]`` ->
     ({action: [ndarray(rows, 7)]}, {action: trajectory id}) exactly as the reference's calc_vel_profile returns them
@@ -179,7 +185,7 @@ class Graph_LTPL(object):
             return self.__calc_paths_next(prev_action_id, object_list, blocked_zones)
         self.__last_path_timestamp = self.clock()   # OTH:395
         sc = ScenarioBatch.from_object_lists([self.__pos], [self.__heading], [self.__start_vel],
-                                             [[o for o in (object_list or []) if o.get('type') == 'physical']],
+                                             [physical_objects(object_list)],
                                              blocked_zones=[blocked_zones] if blocked_zones else None)
         for o in (object_list or []):
             if o.get('type') != 'physical':   # OLI:140-141
@@ -209,7 +215,7 @@ class Graph_LTPL(object):
         self.__calc_buffer.append(calc_time)
         t_const = min(float(np.sum(self.__calc_buffer) / len(self.__calc_buffer)) * 2.0, 0.5)
         sc = ScenarioBatch.from_object_lists([self.__pos], [self.__heading], [self.__start_vel],
-                                             [[o for o in (object_list or []) if o.get('type') == 'physical']],
+                                             [physical_objects(object_list)],
                                              blocked_zones=[blocked_zones] if blocked_zones else None)
         # 'emergency': the device translates it to the action its profile was based on (OTH:307-309)
         sel = dict({v: k for k, v in capi.ACTION_NAMES.items()}, emergency=capi.ACT_EMERGENCY)[prev_action_id]

@@ -12,10 +12,9 @@ import os
 import subprocess
 import sys
 
-ABI_VERSION = 15
+ABI_VERSION = 16
 MAX_SUB = 8
 NSLOT = 3
-KMAX = 16
 MAX_AXM = 32
 
 ACT_NONE, ACT_STRAIGHT, ACT_FOLLOW, ACT_LEFT, ACT_RIGHT = -1, 0, 1, 2, 3
@@ -91,9 +90,9 @@ class VelBatch(C.Structure):
                 ("v_start", C.c_void_p), ("v_end", C.c_void_p), ("vx", C.c_void_p), ("ax", C.c_void_p)]
 
 
-EXPORTS = ("ltpl_version", "ltpl_last_error", "ltpl_sizeof", "ltpl_lattice_create", "ltpl_lattice_destroy",
-           "ltpl_set_startpos_batch", "ltpl_calc_paths_batch", "ltpl_calc_vel_profile_batch", "ltpl_tick_batch",
-           "ltpl_velprofile_batch", "ltpl_launch_count", "ltpl_launch_stage", "ltpl_next_tick_batch",
+EXPORTS = ("ltpl_version", "ltpl_last_error", "ltpl_sizeof", "ltpl_max_objects", "ltpl_lattice_create",
+           "ltpl_lattice_destroy", "ltpl_set_startpos_batch", "ltpl_calc_paths_batch", "ltpl_calc_vel_profile_batch",
+           "ltpl_tick_batch", "ltpl_velprofile_batch", "ltpl_launch_count", "ltpl_launch_stage", "ltpl_next_tick_batch",
            "ltpl_next_calc_paths_batch", "ltpl_next_calc_vel_profile_batch", "ltpl_set_subbatches")
 
 
@@ -136,6 +135,8 @@ def load_library():
     lib.ltpl_launch_count.restype = C.c_uint64
     lib.ltpl_lattice_create.argtypes = [C.POINTER(LatticeHeader), C.c_void_p, C.POINTER(C.c_void_p)]
     lib.ltpl_lattice_destroy.argtypes = [C.c_void_p]
+    lib.ltpl_max_objects.argtypes = [C.POINTER(LatticeHeader), C.c_int]
+    lib.ltpl_max_objects.restype = C.c_int
     lib.ltpl_set_subbatches.argtypes = [C.c_void_p, C.c_int]
     lib.ltpl_set_subbatches.restype = C.c_int
     for fn in (lib.ltpl_set_startpos_batch, lib.ltpl_calc_paths_batch, lib.ltpl_calc_vel_profile_batch,

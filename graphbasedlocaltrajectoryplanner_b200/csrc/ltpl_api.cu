@@ -49,12 +49,13 @@ static const int kThreads = LTPL_WARPS_PER_CTA * 32;
 // device and is shared by every handle and thread there, so it is only ever raised (another handle may rely on a larger
 // value), under a lock.  The size a handle has made sure of is kept per handle (one handle, one device) to skip the calls.
 enum SmemFamily { kSmemFollow, kSmemPlan, kSmemPath, kSmemVel };
+static const size_t kSmemCap = 200 * 1024;
 static std::mutex g_smem_lock;
 
 template <class Fn, size_t N>
 static int allow_smem(const LtplLattice* lat, SmemFamily fam, size_t smem, Fn const (&fns)[N], const char* name,
                       const char* too_large) {
-    if (smem > 200 * 1024) return fail(too_large);
+    if (smem > kSmemCap) return fail(too_large);
     if (smem > 48 * 1024 && smem > lat->smem_allowed[fam]) {
         std::lock_guard<std::mutex> lock(g_smem_lock);
         for (Fn f : fns) {
@@ -73,22 +74,55 @@ static int allow_smem(const LtplLattice* lat, SmemFamily fam, size_t smem, Fn co
     return 0;
 }
 
-// k_plan<ZONE, STATE, DENSE>: one warp per scenario (ltpl_plan.cuh)
+// k_plan's per-warp shared memory: node rows of maxn entries, bits of the edge window
+static int plan_maxn(const LtplLatticeHeader* h) { return ((h->max_nodes_per_layer + 31) / 32) * 32; }
+static int plan_mask_words(const LtplLatticeHeader* h) { return (h->max_window_edges + 31) / 32 + 1; }
+
+// largest dims.k_obj whose k_plan shared memory stays within kSmemCap; 0: not even the lattice window fits
+static int max_objects(const LtplLatticeHeader* h, int h_max) {
+    const int maxn = plan_maxn(h), mw = plan_mask_words(h);
+    const size_t per_warp = kSmemCap / LTPL_WARPS_PER_CTA;
+    const size_t base = plan_smem_bytes_per_warp(maxn, h_max, mw, 0);
+    if (base > per_warp) return 0;
+    int k = (int)((per_warp - base) / sizeof(VehRec));
+    while (k > 0 && plan_smem_bytes_per_warp(maxn, h_max, mw, k) > per_warp) --k;
+    return k;
+}
+
+// k_plan<ZONE, STATE, DENSE>: one warp per scenario (ltpl_plan.cuh), [ZONE + 2 STATE + 4 DENSE]
+typedef void (*PlanFn)(const __grid_constant__ LatDev, const __grid_constant__ LtplParams, const __grid_constant__ LtplDims,
+                       const __grid_constant__ LtplBuffers, const int, const int, const int);
+static const PlanFn kPlanFns[8] = {k_plan<false, false, false>, k_plan<true, false, false>, k_plan<false, true, false>,
+                                   k_plan<true, true, false>,   k_plan<false, false, true>, k_plan<true, false, true>,
+                                   k_plan<false, true, true>,   k_plan<true, true, true>};
+
 static int launch_k_plan(const LtplLattice* lat, const LtplParams* prm, const LtplDims* dm, const LtplBuffers* bf,
                          cudaStream_t st, bool stateful) {
-    const int maxn = ((lat->h.max_nodes_per_layer + 31) / 32) * 32;
+    const int maxn = plan_maxn(&lat->h);
     const int hl = dm->h_max;
-    const int mask_words = (lat->h.max_window_edges + 31) / 32 + 1;
-    const size_t smem = plan_smem_bytes_per_warp(maxn, hl, mask_words) * LTPL_WARPS_PER_CTA;
-    typedef void (*PlanFn)(const __grid_constant__ LatDev, const __grid_constant__ LtplParams, const __grid_constant__ LtplDims,
-                           const __grid_constant__ LtplBuffers, const int, const int, const int);
-    static const PlanFn fns[8] = {k_plan<false, false, false>, k_plan<true, false, false>, k_plan<false, true, false>,
-                                  k_plan<true, true, false>,   k_plan<false, false, true>, k_plan<true, false, true>,
-                                  k_plan<false, true, true>,   k_plan<true, true, true>};
-    if (int r = allow_smem(lat, kSmemPlan, smem, fns, "k_plan", "lattice window too large for shared memory")) return r;
+    const int mask_words = plan_mask_words(&lat->h);
+    const size_t smem = plan_smem_bytes_per_warp(maxn, hl, mask_words, dm->k_obj) * LTPL_WARPS_PER_CTA;
+    if (int r = allow_smem(lat, kSmemPlan, smem, kPlanFns, "k_plan", "lattice window too large for shared memory"))
+        return r;
+    // Shared-memory carveout: what LTPL_PLAN_MINB CTAs need with at least 16 object slots (1 KB reserved per CTA, 228 KB
+    // per sm_90 SM).  For fewer slots the driver would pick a smaller carveout (more L1) for k_plan, and the benchmark
+    // then runs about 4 % slower on an H100: k_vel_res of the other scenario windows, which needs the largest carveout,
+    // slows down beside it (DESIGN.md section 5).  The attribute is a hint shared by every handle on the device.
+    const size_t need = (plan_smem_bytes_per_warp(maxn, hl, mask_words, dm->k_obj < 16 ? 16 : dm->k_obj) *
+                         LTPL_WARPS_PER_CTA + 1024) * LTPL_PLAN_MINB;
+    const int carveout = (int)((need * 100 + 228 * 1024 - 1) / (228 * 1024));
+    if (carveout != lat->plan_carveout) {
+        for (PlanFn f : kPlanFns)
+            if (cudaFuncSetAttribute((const void*)f, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                     carveout < 100 ? carveout : 100) != cudaSuccess) {
+                (void)cudaGetLastError();
+                return fail("k_plan: shared-memory carveout attribute");
+            }
+        lat->plan_carveout = carveout;
+    }
     const bool zone = dm->n_zones > 0;
     const bool dense = lat->h.num_edges >= 2 * lat->h.num_nodes;   // in-edges per node (dp_run<.., DENSE>)
-    fns[(zone ? 1 : 0) + (stateful ? 2 : 0) + (dense ? 4 : 0)]<<<ctas(dm->sub_cnt), kThreads, smem, st>>>(
+    kPlanFns[(zone ? 1 : 0) + (stateful ? 2 : 0) + (dense ? 4 : 0)]<<<ctas(dm->sub_cnt), kThreads, smem, st>>>(
         lat->d, *prm, *dm, *bf, maxn, hl, mask_words);
     return check_launch("k_plan");
 }
@@ -145,6 +179,8 @@ int ltpl_sizeof(int which) {
         default: return -1;
     }
 }
+
+int ltpl_max_objects(const LtplLatticeHeader* h, int h_max) { return h ? max_objects(h, h_max) : -1; }
 
 int ltpl_lattice_create(const LtplLatticeHeader* h, void* dev_blob, LtplLattice** out) {
     if (!h || !dev_blob || !out) return fail("ltpl_lattice_create: null argument");
@@ -341,7 +377,16 @@ static int validate(const LtplLattice* lat, const LtplParams* prm, const LtplDim
             if (!ptr[i]) return fail("buffers: a required device pointer is NULL");
     }
     if (dm->h_max < 3 || dm->p0_max < 2 || dm->n_export < 1) return fail("dims: h_max >= 3, p0_max >= 2, n_export >= 1");
-    if (dm->k_obj < 1 || dm->k_obj > LTPL_KMAX) return fail("dims.k_obj must be in [1, 16]");
+    if (dm->k_obj < 1) return fail("dims.k_obj must be >= 1");
+    {   // (a lattice window too large for any object slot is refused by the k_plan launch)
+        const int kmax = max_objects(&lat->h, dm->h_max);
+        if (kmax >= 1 && dm->k_obj > kmax) {
+            char msg[160];
+            snprintf(msg, sizeof(msg), "dims.k_obj: too many object slots for k_plan's shared memory (%d > %d on this "
+                     "lattice at h_max %d)", dm->k_obj, kmax, dm->h_max);
+            return fail(msg);
+        }
+    }
     if (dm->p_max % 4 != 0 || dm->p_max < dm->p0_max) return fail("dims.p_max must be a multiple of 4 and >= p0_max");
     if (prm->n_axm < 1 || prm->n_axm > LTPL_MAX_AXM) return fail("params.n_axm out of range");
     if (dm->k_pred < 0 || (dm->k_pred > 0 && (!bf->obj_pred || !bf->n_pred)))

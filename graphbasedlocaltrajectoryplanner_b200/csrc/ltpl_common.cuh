@@ -92,6 +92,7 @@ struct LtplLattice {
     cudaEvent_t ev_fork = nullptr, ev_join[LTPL_MAX_SUB - 1] = {};
     // dynamic shared memory each kernel family (ltpl_api.cu: SmemFamily) may use on this handle's device
     mutable size_t smem_allowed[4] = {};
+    mutable int plan_carveout = -1;   // k_plan's preferred shared-memory carveout last set by this handle (percent)
 };
 
 // scenario of a one-warp-per-scenario kernel inside the launch's sub-batch window (-1: none)

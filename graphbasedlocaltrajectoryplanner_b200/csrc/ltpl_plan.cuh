@@ -3,7 +3,6 @@
 #pragma once
 #include "ltpl_common.cuh"
 
-#define LTPL_KMAX 16          // object slots per scenario held in shared memory
 #define LTPL_DMAX 32          // obstacle discs per chunk of the disc stage (one warp ballot; a scenario may hold any number)
 #define LTPL_WARPS_PER_CTA 4
 
@@ -440,23 +439,35 @@ __device__ __forceinline__ int dp_goal(const LatDev& lt, int lane, const DpCtx& 
 // ---------------------------------------------------------------------------------------------------------------------
 // k_plan: OLI.process_object_list + gen_local_node_template + main_online_path_gen (action sets + graph search)
 // ---------------------------------------------------------------------------------------------------------------------
-struct PlanSmem {  // per warp, followed by dist / mask / pred (sizes depend on the lattice)
-    double vx[LTPL_KMAX], vy[LTPL_KMAX], vr[LTPL_KMAX], vv[LTPL_KMAX];
-    double vref[LTPL_KMAX];               // inflated disc radius, squared (GB:626-629)
-    double vpx[LTPL_KMAX], vpy[LTPL_KMAX]; // built-in 0.2 s prediction point of a vehicle without a 'prediction' array
+struct PlanSmem {  // per warp, followed by dist / mask / pred (sizes depend on the lattice) and the vehicle records
     // obstacle discs (GLNT:169-189): per on-track vehicle its current position followed by its prediction points; the
     // discs of a scenario are numbered in that order and visited in chunks of 32, disc c0 + l of a chunk at index l
     double dx[LTPL_DMAX], dy[LTPL_DMAX], dref[LTPL_DMAX];
-    int vd0[LTPL_KMAX], vdn[LTPL_KMAX];   // first disc of a vehicle, number of prediction discs behind it
-    int vslot[LTPL_KMAX];                 // object slot of the vehicle's obj_pred row, -1: built-in 0.2 s point
-    int vlayer[LTPL_KMAX];                // layer of the vehicle's last disc (-1: outside the planning range), q14
+    double s_seg[2];      // race-line s coordinates of the start and the end of the constant path segment
 };
 
-// per warp: PlanSmem | dist f64[2 maxn] | dsave f64[maxn] | meta int4[hl] | mask u32[mask_words] | pred u8[hl maxn]
-__host__ __device__ inline size_t plan_smem_bytes_per_warp(int maxn, int hl, int mask_words) {
+// one on-track object ("vehicle"), in the order of the object list; a warp holds dims.k_obj of them
+struct VehRec {
+    double x, y, r, v;
+    double ref;           // inflated disc radius, squared (GB:626-629)
+    double px, py;        // built-in 0.2 s prediction point of a vehicle without a 'prediction' array (until k_plan
+                          // computes it after the object chunks, px holds the heading)
+    double s;             // race-line s coordinate of the position (constant-segment check, MOPG:90-97)
+    int d0, dn;           // first disc of the vehicle, number of prediction discs behind it
+    int slot;             // object slot of the vehicle's obj_pred row, -1: built-in 0.2 s point
+    int layer;            // layer of the vehicle's last disc (-1: outside the planning range), q14
+};
+
+// per warp: PlanSmem | dist f64[2 maxn] | dsave f64[maxn] | meta int4[hl] | mask u32[mask_words] | pred u8[hl maxn] |
+// VehRec[k_obj] (last: the offsets of everything else do not depend on k_obj)
+__host__ __device__ inline size_t plan_veh_offset(int maxn, int hl, int mask_words) {
     size_t s = sizeof(PlanSmem) + sizeof(double) * 3 * (size_t)maxn + sizeof(int4) * (size_t)hl +
                sizeof(unsigned) * mask_words + (size_t)hl * maxn;
     return (s + 15) & ~(size_t)15;
+}
+
+__host__ __device__ inline size_t plan_smem_bytes_per_warp(int maxn, int hl, int mask_words, int k_obj) {
+    return plan_veh_offset(maxn, hl, mask_words) + ((sizeof(VehRec) * (size_t)k_obj + 15) & ~(size_t)15);
 }
 
 // mark edges of layer pair a -> a+1 that hold a sample inside one of the inflated obstacle discs in `discs` (bit d ->
@@ -526,46 +537,101 @@ __device__ __forceinline__ int disc_pairs(const LatDev& lt, int o, int p_start, 
     return o;
 }
 
+// One chunk of k_plan's object stage (OLI:96-141; object slots c0 .. c0 + 31 of the scenario, lane l = slot c0 + l):
+// on-track test, radius, prediction points -- the caller's 'prediction' array (OLI:117-119) or one constant-velocity
+// point at 0.2 s (OLI:121-127) -- and the race-line s coordinate of a vehicle past the first 30.  The on-track objects
+// keep their list order: vehicle n_veh + (on-track objects of the chunk in front), first disc n_disc + (their discs in
+// front).  Returns the counts after the chunk.  Out of line: the warp-wide fallback of lanes_closest_point is a call,
+// and inside k_plan's chunk loop every value live across it would take a spill slot.
+__device__ __noinline__ int2 chunk_objects(const LatDev& lt, const LtplDims& dm, const LtplBuffers& bf, VehRec* vr,
+                                           int b, int c0, int n_in, int n_veh, int n_disc, int lane) {
+    const int k = c0 + lane;
+    const bool act = k < n_in;
+    const double* o = bf.obj + ((size_t)b * dm.k_obj + (act ? k : 0)) * 5;
+    const double ox = o[0], oy = o[1];
+    const int nb = lanes_closest_point(lt, lt.grid_center, lt.center, lt.L, ox, oy, act, lane);
+    const bool inside = act && inside_bounds_from_vertex(lt, nb, ox, oy);
+    const unsigned in_mask = __ballot_sync(LTPL_FULL, inside);
+    int np_k = -1;   // -1: built-in prediction
+    if (inside && dm.k_pred > 0 && bf.n_pred) np_k = min(bf.n_pred[(size_t)b * dm.k_obj + k], dm.k_pred);
+    const int n_pd = (np_k < 0) ? 1 : np_k;
+    const int mine = inside ? 1 + n_pd : 0;
+    int incl = mine;   // inclusive prefix sum of the disc counts
+#pragma unroll
+    for (int off = 1; off < 32; off <<= 1) {
+        const int up = __shfl_up_sync(LTPL_FULL, incl, off);
+        if (lane >= off) incl += up;
+    }
+    if (inside) {
+        VehRec& w = vr[n_veh + __popc(in_mask & ((1u << lane) - 1u))];
+        const double th = o[2], v = o[3], r = o[4] / 2.0;
+        w.x = ox;
+        w.y = oy;
+        w.r = r;
+        w.v = v;
+        w.px = th;   // the heading, until k_plan replaces it with the built-in point
+        w.d0 = n_disc + incl - mine;
+        w.dn = n_pd;
+        w.slot = (np_k < 0) ? -1 : k;
+        // obstacle_ref = (r + veh_width / 2)^2 + stepsize^2 / 4  (GB:626-629)
+        w.ref = __dadd_rn(sq_rn(__dadd_rn(r, __ddiv_rn(lt.veh_width, 2.0))), __ddiv_rn(sq_rn(lt.step), 4.0));
+    }
+    // race-line s coordinate of a vehicle past the first 30, for the constant-segment check (MOPG:90-97; k_plan
+    // queries those of vehicles 0 .. 29 together with the segment ends)
+    const int v_i = n_veh + __popc(in_mask & ((1u << lane) - 1u));
+    const bool late = inside && v_i >= 30;
+    if (__any_sync(LTPL_FULL, late)) {
+        const int q_nb = lanes_closest_point(lt, lt.grid_raceline, lt.raceline, lt.L, ox, oy, late, lane);
+        if (late) vr[v_i].s = s_coord_from_vertex(lt.raceline, lt.s_rl, lt.L, q_nb, ox, oy);
+    }
+    return make_int2(n_veh + __popc(in_mask), n_disc + __shfl_sync(LTPL_FULL, incl, 31));
+}
+
 // One chunk of k_plan's disc stage (discs c0 .. c0 + 31 of the scenario): lane l materialises disc d = c0 + l into
 // ps->dx / dy / dref[l] and returns the layer pairs it can block, (pa + 1) | (pb + 1) << 16 (disc_pairs, 0: none); the
-// layer of every vehicle whose last disc lies in the chunk goes to ps->vlayer (q14).  Out of line: the warp-wide
-// fallback of lanes_closest_point is a call, and inside k_plan's chunk loop every value live across it would take a
-// spill slot.
+// layer of every vehicle whose last disc lies in the chunk goes to its record (q14).  Out of line like chunk_objects.
 __device__ __noinline__ int chunk_discs(const LatDev& lt, const LtplDims& dm, const LtplBuffers& bf, PlanSmem* ps,
-                                        int b, int c0, int n_disc, int n_veh, int start_layer, int end_layer, int lane) {
+                                        VehRec* vr, int b, int c0, int n_disc, int n_veh, int start_layer, int end_layer,
+                                        int lane) {
     const int d = c0 + lane;
     const bool act = d < n_disc;
     double ox = 0.0, oy = 0.0;
+    int v = 0, j = -1;
     if (act) {
-        // vehicle of disc d: the last one whose first disc is <= d; position j = 0, then its prediction points
-        int v = 0;
+        // vehicle of disc d: the last one whose first disc is <= d (the first discs increase with the vehicle index:
+        // every vehicle has at least its current position); position j = 0, then its prediction points
+        int hi = n_veh - 1;
         #pragma unroll 1
-        for (int w = 1; w < n_veh; ++w)
-            if (ps->vd0[w] <= d) v = w;
-        const int j = d - ps->vd0[v], slot = ps->vslot[v];
+        while (v < hi) {
+            const int mid = (v + hi + 1) >> 1;
+            if (vr[mid].d0 <= d)
+                v = mid;
+            else
+                hi = mid - 1;
+        }
+        const VehRec& w = vr[v];
+        j = d - w.d0;
         if (j == 0) {
-            ox = ps->vx[v];
-            oy = ps->vy[v];
-        } else if (slot < 0) {
-            ox = ps->vpx[v];
-            oy = ps->vpy[v];
+            ox = w.x;
+            oy = w.y;
+        } else if (w.slot < 0) {
+            ox = w.px;
+            oy = w.py;
         } else {
-            const double* pp = bf.obj_pred + (((size_t)b * dm.k_obj + slot) * dm.k_pred + (j - 1)) * 2;
+            const double* pp = bf.obj_pred + (((size_t)b * dm.k_obj + w.slot) * dm.k_pred + (j - 1)) * 2;
             ox = pp[0];
             oy = pp[1];
         }
         ps->dx[lane] = ox;
         ps->dy[lane] = oy;
-        ps->dref[lane] = ps->vref[v];
+        ps->dref[lane] = w.ref;
     }
     const int o = lanes_closest_point(lt, lt.grid_refline, lt.refline, lt.L, ox, oy, act, lane);
     int pa = -1, pb = -1;
     if (act) {
         const int layer = disc_pairs(lt, o, start_layer, end_layer, &pa, &pb);
         // current position, then the prediction points: the LAST one sets obj_layer (q14)
-        #pragma unroll 1
-        for (int w = 0; w < n_veh; ++w)
-            if (ps->vd0[w] + ps->vdn[w] == d) ps->vlayer[w] = layer;
+        if (j == vr[v].dn) vr[v].layer = layer;
     }
     return (pa + 1) | ((pb + 1) << 16);
 }
@@ -594,8 +660,9 @@ k_plan(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm
     const int wib = threadIdx.x >> 5;
     const int b = sub_scenario(dm, LTPL_WARPS_PER_CTA);
     if (b < 0) return;
-    unsigned char* base = smem_raw + plan_smem_bytes_per_warp(maxn, hl, mask_words) * wib;
+    unsigned char* base = smem_raw + plan_smem_bytes_per_warp(maxn, hl, mask_words, dm.k_obj) * wib;
     PlanSmem* ps = reinterpret_cast<PlanSmem*>(base);
+    VehRec* vr = reinterpret_cast<VehRec*>(base + plan_veh_offset(maxn, hl, mask_words));
     double* dist = reinterpret_cast<double*>(base + sizeof(PlanSmem));
     double* dsave = dist + 2 * maxn;
     int4* meta = reinterpret_cast<int4*>(dsave + maxn);
@@ -624,47 +691,61 @@ k_plan(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm
     // entries of the node / node-index / coefficient lists in front of the start node
     const int cnd = STATE ? bf.st_info[8 * (size_t)b + 3] : 1;
 
-    // ---- OLI.process_object_list (OLI:96-141): drop off-track objects, radius = length / 2, prediction points: the
-    // caller's 'prediction' array (OLI:117-119) or one constant-velocity point at 0.2 s (OLI:121-127) ----
+    // ---- OLI.process_object_list (OLI:96-141): drop off-track objects, radius = length / 2, prediction points; the
+    // object slots in chunks of 32 ----
     int n_veh = 0, n_disc = 0;
     {
-        int n_in = bf.n_obj[b];
-        if (n_in > dm.k_obj) n_in = dm.k_obj;
-        // lane k = object k (k_obj <= 16): on-track test, radius, discs -- all objects at once; the on-track objects keep
-        // their order (vehicle index = number of on-track objects in front, disc index = their discs in front)
-        const bool act = lane < n_in;
-        const double* o = bf.obj + ((size_t)b * dm.k_obj + (act ? lane : 0)) * 5;
-        const double ox = o[0], oy = o[1];
-        const int nb = lanes_closest_point(lt, lt.grid_center, lt.center, lt.L, ox, oy, act, lane);
-        const bool inside = act && inside_bounds_from_vertex(lt, nb, ox, oy);
-        const unsigned in_mask = __ballot_sync(LTPL_FULL, inside);
-        int np_k = -1;   // -1: built-in prediction
-        if (inside && dm.k_pred > 0 && bf.n_pred) np_k = min(bf.n_pred[(size_t)b * dm.k_obj + lane], dm.k_pred);
-        const int n_pd = (np_k < 0) ? 1 : np_k;
-        const int mine = inside ? 1 + n_pd : 0;
-        int incl = mine;   // inclusive prefix sum of the disc counts
-#pragma unroll
-        for (int off = 1; off < 32; off <<= 1) {
-            const int up = __shfl_up_sync(LTPL_FULL, incl, off);
-            if (lane >= off) incl += up;
+        const int n_in = min(bf.n_obj[b], dm.k_obj);
+        #pragma unroll 1
+        for (int c0 = 0; c0 < n_in; c0 += 32) {
+            const int2 cnt = chunk_objects(lt, dm, bf, vr, b, c0, n_in, n_veh, n_disc, lane);
+            n_veh = cnt.x;
+            n_disc = cnt.y;
         }
-        n_disc = __shfl_sync(LTPL_FULL, incl, 31);
-        n_veh = __popc(in_mask);
-        if (inside) {
-            const int v_i = __popc(in_mask & ((1u << lane) - 1u));
-            const double th = o[2], v = o[3], r = o[4] / 2.0;
-            ps->vx[v_i] = ox;
-            ps->vy[v_i] = oy;
-            ps->vr[v_i] = r;
-            ps->vv[v_i] = v;
-            ps->vd0[v_i] = incl - mine;
-            ps->vdn[v_i] = n_pd;
-            ps->vslot[v_i] = (np_k < 0) ? -1 : lane;
-            // obstacle_ref = (r + veh_width / 2)^2 + stepsize^2 / 4  (GB:626-629)
-            ps->vref[v_i] = __dadd_rn(sq_rn(__dadd_rn(r, __ddiv_rn(lt.veh_width, 2.0))), __ddiv_rn(sq_rn(lt.step), 4.0));
-            if (np_k < 0) {
-                ps->vpx[v_i] = __dsub_rn(ox, __dmul_rn(__dmul_rn(sin(th), v), 0.2));
-                ps->vpy[v_i] = __dadd_rn(oy, __dmul_rn(__dmul_rn(cos(th), v), 0.2));
+    }
+    __syncwarp();
+    {   // race-line s coordinates for the constant-segment check (MOPG:80-97), one query: lane 0 the start, lane 1 the
+        // end of the constant segment, lane 2 + v vehicle v < 30 (the later ones: chunk_objects)
+        const int p0 = bf.const_len[b];
+        size_t cplane = (size_t)dm.batch * dm.p0_max;
+        const double* cs = bf.const_seg + (size_t)b * dm.p0_max;
+        if (STATE) {
+            const int* sinfo = bf.st_info + 8 * (size_t)b;
+            cplane = (size_t)LTPL_NSLOT * dm.batch * dm.p_max;
+            cs = bf.prev_path + (size_t)sinfo[0] * dm.p_max + sinfo[1];
+        }
+        double qx = 0.0, qy = 0.0;
+        bool q_act = false;
+        if (p0 >= 2) {
+            q_act = lane < 2 + n_veh;
+            if (lane == 0) {   // MOPG:80-84: pos_est of the previous calc_vel_profile call; None on the first tick
+                qx = STATE ? bf.pos_last[2 * b] : cs[0];
+                qy = STATE ? bf.pos_last[2 * b + 1] : cs[cplane];
+            } else if (lane == 1) {
+                qx = cs[p0 - 1];
+                qy = cs[cplane + p0 - 1];
+            } else if (q_act) {
+                qx = vr[lane - 2].x;
+                qy = vr[lane - 2].y;
+            }
+        }
+        const int q_nb = lanes_closest_point(lt, lt.grid_raceline, lt.raceline, lt.L, qx, qy, q_act, lane);
+        if (q_act) {
+            const double sq = s_coord_from_vertex(lt.raceline, lt.s_rl, lt.L, q_nb, qx, qy);
+            if (lane < 2)
+                ps->s_seg[lane] = sq;
+            else
+                vr[lane - 2].s = sq;
+        }
+    }
+    {   // the built-in 0.2 s point (OLI:121-127); the float64 sin / cos stay here, out of the chunk functions' frames
+        #pragma unroll 1
+        for (int v = lane; v < n_veh; v += 32) {
+            VehRec& w = vr[v];
+            if (w.slot < 0) {
+                const double th = w.px;
+                w.px = __dsub_rn(w.x, __dmul_rn(__dmul_rn(sin(th), w.v), 0.2));
+                w.py = __dadd_rn(w.y, __dmul_rn(__dmul_rn(cos(th), w.v), 0.2));
             }
         }
     }
@@ -689,7 +770,7 @@ k_plan(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm
     __syncwarp();
     #pragma unroll 1
     for (int c0 = 0; c0 < n_disc; c0 += LTPL_DMAX) {
-        const int pr = chunk_discs(lt, dm, bf, ps, b, c0, n_disc, n_veh, start_layer, end_layer, lane);  // lane l: disc c0 + l
+        const int pr = chunk_discs(lt, dm, bf, ps, vr, b, c0, n_disc, n_veh, start_layer, end_layer, lane);  // lane l: disc c0 + l
         __syncwarp();
         #pragma unroll 1
         for (int dl = 0; dl < LTPL_DMAX && c0 + dl < n_disc; ++dl) {  // one sweep per distinct layer pair of the chunk
@@ -705,23 +786,31 @@ k_plan(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm
         }
         __syncwarp();
     }
-    #pragma unroll 1
-    for (int v = 0; v < n_veh; ++v) {
-        const int obj_layer = ps->vlayer[v];
-        if (obj_layer >= 0) {
-            int ld = obj_layer - start_layer;
-            if (ld < 0) ld = lt.L - start_layer + obj_layer;
-            if (ld <= planning_dist && (closest_dist < 0 || ld < closest_dist)) {
-                closest_dist = ld;
-                closest_idx = v;
-                con_layer = obj_layer;
+    {   // the first vehicle with the strictly smallest layer distance (GLNT:194-204), each lane over every 32nd vehicle
+        int best_ld = 0x7fffffff, best_v = 0x7fffffff;
+        #pragma unroll 1
+        for (int v = lane; v < n_veh; v += 32) {
+            const int obj_layer = vr[v].layer;
+            if (obj_layer >= 0) {
+                int ld = obj_layer - start_layer;
+                if (ld < 0) ld = lt.L - start_layer + obj_layer;
+                if (ld <= planning_dist && ld < best_ld) {
+                    best_ld = ld;
+                    best_v = v;
+                }
             }
+        }
+        const int m_ld = __reduce_min_sync(LTPL_FULL, (unsigned)best_ld);
+        if (m_ld != 0x7fffffff) {
+            closest_dist = m_ld;
+            closest_idx = __reduce_min_sync(LTPL_FULL, (best_ld == m_ld) ? (unsigned)best_v : 0x7fffffffu);
+            con_layer = vr[closest_idx].layer;
         }
     }
     if (closest_dist >= 0) {  // GLNT:206-213
         const int nb = lt.node_off[con_layer];
-        const ArgMinD m = warp_closest_point(lt.node_xy + nb, lt.node_off[con_layer + 1] - nb, ps->vx[closest_idx],
-                                             ps->vy[closest_idx], lane);
+        const ArgMinD m = warp_closest_point(lt.node_xy + nb, lt.node_off[con_layer + 1] - nb, vr[closest_idx].x,
+                                             vr[closest_idx].y, lane);
         con_node = m.i;
     }
     LTPL_PH(18)
@@ -739,27 +828,11 @@ k_plan(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm
     }
     bool obj_in_const = false, obj_beside = false;
     if (p0 >= 2) {
-        // MOPG:80-84: pos_est of the previous calc_vel_profile call; None on the first tick -> first point of the segment
-        const double sx0 = STATE ? bf.pos_last[2 * b] : cs[0], sy0 = STATE ? bf.pos_last[2 * b + 1] : cs[cplane];
-        const double sxe = cs[p0 - 1], sye = cs[cplane + p0 - 1];
-        // s coordinates on the race line: lane 0 the start, lane 1 the end of the segment, lane 2 + v object v (n_veh <= 16)
-        double qx = sx0, qy = sy0;
-        if (lane == 1) {
-            qx = sxe;
-            qy = sye;
-        } else if (lane >= 2 && lane - 2 < n_veh) {
-            qx = ps->vx[lane - 2];
-            qy = ps->vy[lane - 2];
-        }
-        const bool q_act = lane < 2 + n_veh;
-        const int q_nb = lanes_closest_point(lt, lt.grid_raceline, lt.raceline, lt.L, qx, qy, q_act, lane);
-        const double s_mine = q_act ? s_coord_from_vertex(lt.raceline, lt.s_rl, lt.L, q_nb, qx, qy) : 0.0;
-        const double s_start = __shfl_sync(LTPL_FULL, s_mine, 0), s_end = __shfl_sync(LTPL_FULL, s_mine, 1);
+        const double s_start = ps->s_seg[0], s_end = ps->s_seg[1];
         double smallest = LTPL_INF;
         #pragma unroll 1
-        for (int v = 0; v < n_veh; ++v) {
-            const double ox = ps->vx[v], oy = ps->vy[v];
-            const double s_obj = __shfl_sync(LTPL_FULL, s_mine, 2 + v);
+        for (int v = 0; v < n_veh; ++v) {   // in list order: quirk q15 depends on it
+            const double s_obj = vr[v].s;
             if ((s_start <= s_obj && s_obj <= s_end) || (s_start > s_end && (s_obj > s_start || s_obj < s_end))) {
                 obj_beside = true;
                 double od;
@@ -771,7 +844,8 @@ k_plan(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm
                     closest_idx = v;
                     smallest = od;
                 }
-                const double oref = sq_rn(__dadd_rn(ps->vr[v], __ddiv_rn(lt.veh_width, 2.0)));
+                const double ox = vr[v].x, oy = vr[v].y;
+                const double oref = sq_rn(__dadd_rn(vr[v].r, __ddiv_rn(lt.veh_width, 2.0)));
                 int hit = 0;
                 #pragma unroll 1
                 for (int k = lane; k < p0; k += 32) hit |= (dist2_rn(cs[k], cs[cplane + k], ox, oy) <= oref) ? 1 : 0;
@@ -784,7 +858,7 @@ k_plan(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm
     // (CVPF:166-172) -- warp-parallel here instead of a serial 800-point scan per follow path in the velocity kernel
     if (closest_idx >= 0) {
         const int ng = lt.n_glob - 1;
-        const double ox = ps->vx[closest_idx], oy = ps->vy[closest_idx];
+        const double ox = vr[closest_idx].x, oy = vr[closest_idx].y;
         const ArgMinD m = warp_closest_point_grid(lt, lt.grid_glob, lt.glob_xy, ng, ox, oy, lane);
         const int nb = m.i;
         const int i1 = (nb - 1 < 0) ? ng - 1 : nb - 1;
@@ -796,9 +870,9 @@ k_plan(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm
     if (lane == 0) {
         bf.closest_obj[b] = closest_idx;
         if (closest_idx >= 0) {
-            bf.cobj[4 * b + 0] = ps->vx[closest_idx];
-            bf.cobj[4 * b + 1] = ps->vy[closest_idx];
-            bf.cobj[4 * b + 2] = ps->vv[closest_idx];
+            bf.cobj[4 * b + 0] = vr[closest_idx].x;
+            bf.cobj[4 * b + 1] = vr[closest_idx].y;
+            bf.cobj[4 * b + 2] = vr[closest_idx].v;
             bf.cobj[4 * b + 3] = 1.0;
         }
     }

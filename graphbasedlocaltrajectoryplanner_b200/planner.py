@@ -36,6 +36,21 @@ def check_filt_window(w) -> int:
     return int(w)
 
 
+def max_objects(header, cap: dict) -> int:
+    """largest object list per scenario a planner over this lattice header and these capacities can plan: k_plan keeps
+    one record per on-track object in shared memory (ltpl_max_objects; several hundred on every lattice)."""
+    return int(capi.load_library().ltpl_max_objects(C.byref(header), int(cap["h_max"])))
+
+
+def check_object_count(k_obj: int, bound: int) -> int:
+    """object slots per scenario: at least 1, at most ``bound`` (max_objects); refused before anything is launched."""
+    k_obj = max(1, int(k_obj))
+    if k_obj > bound:
+        raise ValueError("%d objects per scenario exceed k_plan's shared memory on this lattice: at most %d"
+                         % (k_obj, bound))
+    return k_obj
+
+
 def read_online_config(path: str) -> dict:
     """online ini keys the batched path needs (reference: OTH:99-122, LTPL:168-173)."""
     cfg = configparser.ConfigParser()
@@ -92,6 +107,7 @@ class BatchPlanner(object):
         self._stateful = bool(stateful)
         if stateful:   # stateful ticks carry constant nodes / points of earlier ticks in front of the new plan
             self.cap = dict(self.cap, h_max=self.cap["h_max"] + 8, p_max=self.cap["p_max"] + 96)
+        self.max_objects = max_objects(self.header, self.cap)
         handle = C.c_void_p()
         capi.check(self.lib, self.lib.ltpl_lattice_create(C.byref(self.header), C.c_void_p(self.blob.data_ptr()),
                                                           C.byref(handle)), "ltpl_lattice_create")
@@ -220,9 +236,7 @@ class BatchPlanner(object):
                 setattr(self.buf, name, views[name].data_ptr())
 
     def allocate(self, batch: int, k_obj: int = 3, k_pred: int = 0) -> None:
-        k_obj = max(1, int(k_obj))
-        if k_obj > capi.KMAX:
-            raise ValueError("at most %d objects per scenario" % capi.KMAX)
+        k_obj = check_object_count(k_obj, self.max_objects)
         if self.dims is not None and self.dims.batch == batch:
             if self.dims.k_obj >= k_obj and self._k_pred_cap >= k_pred:
                 return
@@ -535,6 +549,7 @@ class BatchPlanner(object):
         if sc.size != self.dims.batch:
             raise ValueError("stateful tick: the batch size must not change within a session (re-anchor with "
                              "set_startpos on a new batch)")
+        check_object_count(sc.obj.shape[1], self.max_objects)   # before the swaps below: a refused list changes nothing
         if self._state is None:
             self._alloc_state()
         st, t, buf = self._state, self.t, self.buf

@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define LTPL_ABI_VERSION 15
+#define LTPL_ABI_VERSION 16
 
 /* action ids (OTH:14-17 ACTION_ID_MAP) */
 #define LTPL_ACT_NONE (-1)
@@ -167,7 +167,8 @@ typedef struct LtplParams {
 /* capacities chosen by the host from the lattice (see lattice_blob.py: capacities()) */
 typedef struct LtplDims {
     int32_t batch;     /* B scenarios                                                  */
-    int32_t k_obj;     /* K object slots per scenario                                  */
+    int32_t k_obj;     /* K object slots per scenario (any number; k_plan holds one record per on-track object  */
+                       /* in shared memory, so it is bounded by ltpl_max_objects, several hundred)               */
     int32_t p0_max;    /* points of the constant segment (pose -> start node)          */
     int32_t p_max;     /* points of a full path (constant segment + new plan), % 4 == 0 */
     int32_t h_max;     /* nodes of a node sequence incl. the leading [None, None] entry */
@@ -301,6 +302,9 @@ int ltpl_sizeof(int which); /* 0 header, 1 params, 2 dims, 3 buffers, 4 velbatch
 /* stream, synchronised before returning) -- the blob is read-only afterwards.                                         */
 int ltpl_lattice_create(const LtplLatticeHeader* header, void* dev_blob, LtplLattice** out);
 int ltpl_lattice_destroy(LtplLattice* lat);
+/* largest dims.k_obj a tick on this lattice header with this dims.h_max accepts (k_plan keeps a record per on-track     */
+/* object in shared memory); 0: none (the lattice window alone is too large), -1: null header.  Needs no device.        */
+int ltpl_max_objects(const LtplLatticeHeader* header, int h_max);
 
 /* Graph_LTPL.set_startpos (LTPL:262-296 -> OTH.set_initial_pose OTH:181-270), batched                                   */
 int ltpl_set_startpos_batch(const LtplLattice* lat, const LtplParams* prm, const LtplDims* dims, const LtplBuffers* buf,

@@ -1,5 +1,6 @@
 """Per-kernel device time of the planning tick (torch.profiler, CUDA activities), GPU box:
     python tools/gpu_kernel_share.py [--lattice l216] [--batch 10000] [--filt-window 5] [--ticks 20] [--stateful]
+                                     [--pred-points N] [--objects N]
 Prints one JSON line: the card, its power limit, and per kernel the time per tick and the share of all kernel time."""
 import argparse
 import json
@@ -11,6 +12,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import torch  # noqa: E402
 
+from bench_objects import with_objects  # noqa: E402
 from bench_pred import with_predictions  # noqa: E402
 from torch.profiler import ProfilerActivity, profile  # noqa: E402
 
@@ -25,13 +27,15 @@ ap.add_argument("--filt-window", type=int, default=1)
 ap.add_argument("--ticks", type=int, default=20)
 ap.add_argument("--stateful", action="store_true", help="time stateful ticks (next_tick) instead of first ticks")
 ap.add_argument("--pred-points", type=int, default=0, help="N-point prediction array on every object (bench_pred.py)")
+ap.add_argument("--objects", type=int, default=0, help="objects filled up to N per scenario (bench_objects.py)")
 args = ap.parse_args()
 
 card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], stdout=subprocess.PIPE,
                       text=True).stdout.strip().splitlines()[0]
 g = H.golden("ticks_%s.npz" % args.lattice)
-sc = with_predictions(make_scenarios(Track(H.track_csv_for(args.lattice)), args.batch, seed=12345, n_obj_min=1,
-                                     n_obj_max=3), args.pred_points)
+track = Track(H.track_csv_for(args.lattice))
+sc = with_predictions(with_objects(make_scenarios(track, args.batch, seed=12345, n_obj_min=1, n_obj_max=3), args.objects,
+                                   track), args.pred_points)
 pl = BatchPlanner(H.lattice_for(args.lattice), online=dict(filt_window_width=args.filt_window), device="cuda:0",
                   stateful=args.stateful)
 pl.set_vel_params(ax_max_machines=g["ax_max_machines"], vel_max=100.0, gg_scale=1.0, local_gg=(5.0, 5.0), safety_d=30.0)
@@ -65,6 +69,7 @@ for ev in prof.key_averages():
         per[name] = per.get(name, 0.0) + ev.device_time_total / 1e3 / args.ticks   # ms per tick
 total = sum(per.values())
 print(json.dumps({"card": card, "lattice": args.lattice, "batch": args.batch, "filt_window": args.filt_window,
-                  "stateful": args.stateful, "pred_points": args.pred_points, "kernel_ms_per_tick": round(total, 4),
+                  "stateful": args.stateful, "pred_points": args.pred_points, "objects": args.objects,
+                  "kernel_ms_per_tick": round(total, 4),
                   "kernels": {k: {"ms_per_tick": round(v, 4), "share": round(v / total, 4)}
                               for k, v in sorted(per.items(), key=lambda kv: -kv[1])}}))

@@ -40,6 +40,18 @@ sel = pp.t["action_id"].max(dim=0).values.clamp(min=0).cpu().numpy()
 pp.next_tick(sc, sel_action=sel, t_const=0.1)
 r = pp.records()
 print("long-prediction stateful tick, trajectories:", sum(len(x.get("traj", {})) for x in r))
+# long object lists (k_plan's object stage in chunks of 32, a vehicle record per on-track object): 70 objects per
+# scenario, every second added one beyond the track bounds, a first tick and a stateful tick
+from bench_objects import with_objects  # noqa: E402
+tr = Track(H.TRACK_CSV)
+sc = with_objects(make_scenarios(tr, n, seed=80, n_obj_min=1, n_obj_max=3), 70, tr)
+po = BatchPlanner(H.lattice_for("default"), device="cuda:0", stateful=True)
+po.set_vel_params(ax_max_machines=g["ax_max_machines"], **VEL)
+po.stage_scenarios(sc); po.upload(); po.set_startpos(); po.tick()
+sel = po.t["action_id"].max(dim=0).values.clamp(min=0).cpu().numpy()
+po.next_tick(sc, sel_action=sel, t_const=0.1)
+r = po.records()
+print("70-object stateful tick, trajectories:", sum(len(x.get("traj", {})) for x in r))
 mb =make_velocity_microbench(200, 150, seed=3)
 vx, ax = calc_vel_profile_batch(pl, mb["kappa"], mb["el"], mb["v_start"], mb["v_end"])
 print("dense vx mean", float(np.mean(vx)))
