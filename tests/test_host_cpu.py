@@ -150,18 +150,27 @@ def test_zone_ids_and_masks_of_a_scenario_batch():
 
 def test_nearest_vertex_grid_bounds_the_argmin():
     """lattice_blob.nearest_grid: for random positions around the track the candidates of the position's cell contain
-    np.argmin's answer (first minimum) of the scan over the whole polyline -- closed and open track."""
+    np.argmin's answer (first minimum) of the scan over the whole polyline -- closed and open track, for all four
+    polylines k_plan searches (the centre line of the in-track test included), also on cell edges and corners."""
     from graphbasedlocaltrajectoryplanner_b200 import lattice_blob as LB
     rng = np.random.default_rng(7)
     for tag in ("l216", "open"):
         lat = H.lattice_for(tag)
         LB.pack_lattice(lat)
         g = lat._nearest_grids
-        polys = dict(refline=lat.refline, raceline=lat.raceline, glob=np.ascontiguousarray(lat.glob_rl[:-1, 1:3]))
+        bound1 = lat.refline + lat.normvec * np.expand_dims(lat.w_right, 1)
+        bound2 = lat.refline - lat.normvec * np.expand_dims(lat.w_left, 1)
+        polys = dict(center=(bound1 + bound2) / 2, refline=lat.refline, raceline=lat.raceline,
+                     glob=np.ascontiguousarray(lat.glob_rl[:-1, 1:3]))
         for name, pts in polys.items():
             n = pts.shape[0]
             q = pts[rng.integers(0, n, 4000)] + rng.normal(0.0, 10.0, (4000, 2))
             q[:200] = pts[rng.integers(0, n, 200)]                       # exactly on vertices
+            # on the edges (x0 + 4k or y0 + 4k) and corners of the cells around the polyline
+            snap = lambda v, v0: v0 + LB.GRID_CELL * np.round((v - v0) / LB.GRID_CELL)   # noqa: E731
+            q[200:400, 0] = snap(q[200:400, 0], g["x0"])
+            q[400:600, 1] = snap(q[400:600, 1], g["y0"])
+            q[600:800, 0], q[600:800, 1] = snap(q[600:800, 0], g["x0"]), snap(q[600:800, 1], g["y0"])
             ix = np.floor((q[:, 0] - g["x0"]) / LB.GRID_CELL).astype(int)
             iy = np.floor((q[:, 1] - g["y0"]) / LB.GRID_CELL).astype(int)
             ent = g[name][iy, ix]
