@@ -12,7 +12,7 @@ import os
 import subprocess
 import sys
 
-ABI_VERSION = 16
+ABI_VERSION = 17
 MAX_SUB = 8
 NSLOT = 3
 MAX_AXM = 32
@@ -77,7 +77,7 @@ BUFFER_FIELDS = ("pos", "heading", "vel", "vel_est", "n_obj", "obj", "sc_flags",
                  "n_pred", "prev_path", "prev_path_len", "prev_node_idx", "prev_nodes", "prev_n_nodes", "prev_coeff",
                  "prev_s_vx_ax", "prev_action_id", "prev_traj_len", "prev_trim", "sel_action", "pos_last", "t_const",
                  "st_info", "trim", "vel_plan", "course", "obj_dist", "zone_s0", "em_vx", "prev_em_vx", "prev_em_info",
-                 "gg", "prev_gg")
+                 "gg", "prev_gg", "restart")
 STATE_FIELDS = BUFFER_FIELDS[BUFFER_FIELDS.index("prev_path"):]   # NULL unless a stateful tick is planned
 
 

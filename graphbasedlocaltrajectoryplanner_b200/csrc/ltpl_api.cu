@@ -417,7 +417,7 @@ int ltpl_set_startpos_batch(const LtplLattice* lat, const LtplParams* prm, const
     // a new session on a buffer set with memory: its first tick processes the zones anew (GLNT:43-77)
     if (bf->trim && bf->zone_s0 && cudaMemsetAsync(bf->zone_s0, 0xFF, sizeof(int) * (size_t)dm->batch, st) != cudaSuccess)
         return fail("memset(zone_s0) failed");
-    k_startpos<<<ctas(dm->batch), kThreads, 0, st>>>(lat->d, *prm, *dm, *bf);
+    k_startpos<<<ctas(dm->batch), kThreads, 0, st>>>(lat->d, *prm, *dm, *bf, 0);
     return check_launch("k_startpos");
 }
 
@@ -449,9 +449,13 @@ static int launch_smooth(const LtplParams* prm, const LtplDims* w, const LtplBuf
     return check_launch("k_smooth");
 }
 
-// one scenario window of calc_paths: (k_state ->) k_plan -> k_path
+// one scenario window of calc_paths: (k_startpos of the restarted scenarios -> k_state ->) k_plan -> k_path
 static int paths_window(const LtplLattice* lat, const LtplParams* prm, const LtplDims* w, const LtplBuffers* bf,
                         cudaStream_t st, bool stateful) {
+    if (stateful && bf->restart) {
+        k_startpos<<<ctas(w->sub_cnt), kThreads, 0, st>>>(lat->d, *prm, *w, *bf, 1);
+        if (int r = check_launch("k_startpos")) return r;
+    }
     if (stateful) {
         k_state<<<ctas(w->sub_cnt), kThreads, 0, st>>>(lat->d, *prm, *w, *bf);
         if (int r = check_launch("k_state")) return r;
@@ -530,7 +534,7 @@ int ltpl_tick_batch(const LtplLattice* lat, const LtplParams* prm, const LtplDim
 }
 
 // stateful tick (ltpl_state.cuh):
-//   ltpl_next_calc_paths_batch        k_state -> k_plan<.., true> -> k_path<true>
+//   ltpl_next_calc_paths_batch        (k_startpos masked by buffers.restart ->) k_state -> k_plan<.., true> -> k_path<true>
 //   ltpl_next_calc_vel_profile_batch  k_ref -> k_vel_res<true> -> k_backup -> k_prefix -> k_export
 int ltpl_next_calc_paths_batch(const LtplLattice* lat, const LtplParams* prm, const LtplDims* dm, const LtplBuffers* bf,
                                void* stream) {

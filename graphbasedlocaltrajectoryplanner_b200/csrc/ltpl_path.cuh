@@ -24,7 +24,8 @@ __device__ __forceinline__ void enqueue_path(const LtplBuffers& bf, const LtplDi
 #ifndef LTPL_PATH_MINB
 #define LTPL_PATH_MINB 8
 #endif
-// STATE: stateful tick (ltpl_state.cuh): the constant part and the list prefixes come from the previous tick's buffers
+// STATE: stateful tick (ltpl_state.cuh): the constant part and the list prefixes come from the previous tick's buffers,
+// except for a scenario restarted in this tick (st_info[0] < 0): set_startpos's, as in a first tick
 template <bool STATE>
 __global__ void __launch_bounds__(LTPL_WARPS_PER_CTA * 32, LTPL_PATH_MINB)
 k_path(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm,
@@ -62,7 +63,8 @@ k_path(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm
     const int* mem_ni = nullptr;       // memory node index list (trimmed at L) and its offset m
     const double* mem_cf = nullptr;
     int mem_m = 0, mem_rows = 0;
-    if (STATE) {
+    const bool mem = STATE && bf.st_info[8 * (size_t)b] >= 0;
+    if (mem) {
         const int* sinfo = bf.st_info + 8 * (size_t)b;
         cplane = pplane;
         cs = bf.prev_path + (size_t)sinfo[0] * dm.p_max + sinfo[1];
@@ -83,7 +85,7 @@ k_path(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm
         for (int k = lane; k < p0; k += 32)
             for (int c = 0; c < 5; ++c) pp[c * pplane + k] = cs[c * cplane + k];
         if (lane == 0) {
-            if (STATE) {   // OTH:486-501: memory lists up to and including the start node
+            if (mem) {   // OTH:486-501: memory lists up to and including the start node
                 for (int i = 0; i < cnd; ++i) node_idx[i] = mem_ni[i] - mem_m;
                 for (int i = 0; i < min(cnd + 1, mem_rows) * 8; ++i) coeff[i] = mem_cf[i];
             } else {
@@ -243,13 +245,13 @@ k_path(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm
 
     // ---- stitched bookkeeping (OTH:458-472) ----
     for (int i = lane; i <= nseg; i += 32) node_idx[cnd + i] = nidx[i] + loc;
-    if (STATE) {
+    if (mem) {
         for (int i = lane; i < cnd; i += 32) node_idx[i] = mem_ni[i] - mem_m;
         for (int i = lane; i < cnd * 8; i += 32) coeff[i] = mem_cf[i];
     }
-    if (!STATE && lane < 8) coeff[lane] = bf.const_coeff[(size_t)b * 8 + lane];
+    if (!mem && lane < 8) coeff[lane] = bf.const_coeff[(size_t)b * 8 + lane];
     if (lane == 0) {
-        if (!STATE) node_idx[0] = 0;
+        if (!mem) node_idx[0] = 0;
         bf.path_len[q] = p_tot;
         enqueue_path(bf, dm, q);
     }

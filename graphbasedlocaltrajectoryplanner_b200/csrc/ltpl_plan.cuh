@@ -36,18 +36,21 @@ __device__ __forceinline__ void head_curv(double ax1, double ax2, double ax3, do
     *kappa = (xd * ydd - yd * xdd) * (r * r * r);
 }
 
+// masked == 0: every scenario of the batch (ltpl_set_startpos_batch).  masked == 1: the scenarios of the window dm with
+// bf.restart[b] != 0 (restart inside a stateful tick, in front of k_state); their zones are processed anew (zone_s0).
 __global__ void __launch_bounds__(LTPL_WARPS_PER_CTA * 32)
 k_startpos(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm,
-           const __grid_constant__ LtplDims dm, const __grid_constant__ LtplBuffers bf) {
+           const __grid_constant__ LtplDims dm, const __grid_constant__ LtplBuffers bf, const int masked) {
     const int lane = threadIdx.x & 31;
-    const int b = blockIdx.x * LTPL_WARPS_PER_CTA + (threadIdx.x >> 5);
-    if (b >= dm.batch) return;
+    const int b = masked ? sub_scenario(dm, LTPL_WARPS_PER_CTA) : blockIdx.x * LTPL_WARPS_PER_CTA + (threadIdx.x >> 5);
+    if (b < 0 || b >= dm.batch || (masked && !bf.restart[b])) return;
     const double px = bf.pos[2 * b], py = bf.pos[2 * b + 1], heading = bf.heading[b];
     int flags = 0;
     if (lane == 0) {
         bf.start_node[2 * b] = -1;
         bf.start_node[2 * b + 1] = -1;
         bf.const_len[b] = 0;
+        if (masked && bf.zone_s0) bf.zone_s0[b] = -1;
     }
     if (!inside_bounds(lt, px, py, lane)) {  // OTH:214-219
         if (lane == 0) bf.sc_flags[b] = LTPL_SC_OUT_OF_TRACK;
@@ -649,7 +652,8 @@ __device__ __forceinline__ int act_filter(int acts, int a) { return (acts >> (5 
 #endif
 // STATE: stateful tick (ltpl_state.cuh): start node / constant segment come from k_state, the constant segment lives in
 // the previous tick's path planes, pos_est and the last action id enter the action-set logic, the first edges of the
-// last solution are cheaper
+// last solution are cheaper.  A scenario restarted in this tick (st_info[0] < 0) is planned like a first tick: its
+// constant segment, start node and [(-1, -1), start] node list are what k_startpos has just produced.
 template <bool ZONE, bool STATE = false, bool DENSE = false>
 __global__ void __launch_bounds__(LTPL_WARPS_PER_CTA * 32, LTPL_PLAN_MINB)
 k_plan(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm,
@@ -709,7 +713,8 @@ k_plan(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm
         const int p0 = bf.const_len[b];
         size_t cplane = (size_t)dm.batch * dm.p0_max;
         const double* cs = bf.const_seg + (size_t)b * dm.p0_max;
-        if (STATE) {
+        const bool mem = STATE && bf.st_info[8 * (size_t)b] >= 0;   // constant segment from the memory
+        if (mem) {
             const int* sinfo = bf.st_info + 8 * (size_t)b;
             cplane = (size_t)LTPL_NSLOT * dm.batch * dm.p_max;
             cs = bf.prev_path + (size_t)sinfo[0] * dm.p_max + sinfo[1];
@@ -719,8 +724,8 @@ k_plan(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm
         if (p0 >= 2) {
             q_act = lane < 2 + n_veh;
             if (lane == 0) {   // MOPG:80-84: pos_est of the previous calc_vel_profile call; None on the first tick
-                qx = STATE ? bf.pos_last[2 * b] : cs[0];
-                qy = STATE ? bf.pos_last[2 * b + 1] : cs[cplane];
+                qx = mem ? bf.pos_last[2 * b] : cs[0];
+                qy = mem ? bf.pos_last[2 * b + 1] : cs[cplane];
             } else if (lane == 1) {
                 qx = cs[p0 - 1];
                 qy = cs[cplane + p0 - 1];
@@ -821,7 +826,7 @@ k_plan(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm
     const int p0 = bf.const_len[b];
     size_t cplane = (size_t)B * dm.p0_max;
     const double* cs = bf.const_seg + (size_t)b * dm.p0_max;
-    if (STATE) {
+    if (STATE && bf.st_info[8 * (size_t)b] >= 0) {
         const int* sinfo = bf.st_info + 8 * (size_t)b;
         cplane = (size_t)LTPL_NSLOT * B * dm.p_max;
         cs = bf.prev_path + (size_t)sinfo[0] * dm.p_max + sinfo[1];
@@ -884,7 +889,8 @@ k_plan(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm
         n_act = 1;
         acts = act_entry(0, LTPL_ACT_FOLLOW, 0);
         // last_action_id (MOPG:130): the executed action, 'emergency' already translated by k_state (st_info[0] = its slot)
-        const int last_act = STATE ? bf.prev_action_id[bf.st_info[8 * (size_t)b]] : LTPL_ACT_STRAIGHT;
+        const int pq = STATE ? bf.st_info[8 * (size_t)b] : -1;
+        const int last_act = pq >= 0 ? bf.prev_action_id[pq] : LTPL_ACT_STRAIGHT;
         if (!obj_in_const && (last_act == LTPL_ACT_LEFT || last_act == LTPL_ACT_RIGHT)) {   // MOPG:130-133: keep overtaking
             acts |= act_entry(1, last_act, 1);
             n_act = 2;
@@ -1050,13 +1056,14 @@ k_plan(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm
             if (src == 1) gj = dp_goal(lt, lane, c, &tie, goal_off);
             if (tie) st |= LTPL_ST_TIE_AMBIGUOUS;
             st |= LTPL_ST_FOUND;
-            if (STATE && src != 2) {   // constant nodes in front of the start node: the memory of the last tick (OTH:462-466)
+            const bool mem = STATE && bf.st_info[8 * (size_t)b] >= 0;
+            if (mem && src != 2) {   // constant nodes in front of the start node: the memory of the last tick (OTH:462-466)
                 const int* sinfo = bf.st_info + 8 * (size_t)b;
                 const int* pn = bf.prev_nodes + ((size_t)sinfo[0] * dm.h_max + sinfo[2]) * 2;
                 for (int i = lane; i < 2 * cnd; i += 32) nd[i] = pn[i];
             }
             if (lane == 0) {
-                if (!STATE) {
+                if (!mem) {
                     nd[0] = -1;
                     nd[1] = -1;
                 }
@@ -1099,7 +1106,7 @@ k_plan(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm
         if (!any && bf.const_len[b] > 2) {   // (re-read: p0 is not kept live across the searches)
             const int q = b;
             int* nd = bf.nodes + (size_t)q * dm.h_max * 2;
-            if (STATE) {
+            if (STATE && bf.st_info[8 * (size_t)b] >= 0) {
                 const int* sinfo = bf.st_info + 8 * (size_t)b;
                 const int* pn = bf.prev_nodes + ((size_t)sinfo[0] * dm.h_max + sinfo[2]) * 2;
                 for (int i = 0; i < 2 * cnd; ++i) nd[i] = pn[i];

@@ -60,6 +60,21 @@ k_state(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams pr
     if (b < 0) return;
     const int B = dm.batch;
     int* info = bf.st_info + 8 * (size_t)b;
+    if (bf.restart && bf.restart[b]) {
+        // set_startpos on the live instance (OTH:161-179, 204): k_startpos has just checked the pose and seeded the forced
+        // 'straight' segment; the memory is dropped.  Marker for the later kernels: st_info[0] = -1 -- the constant
+        // segment is set_startpos's, no cost reduction, cut 0 at vel (get_ref_idx without a last trajectory, OTH:592-598),
+        // no backup plan.  A rejected pose keeps the flags k_startpos wrote.
+        if (lane == 0 && bf.sc_flags[b] == 0) {
+            info[0] = -1;
+            info[1] = info[2] = 0;
+            info[3] = 1;                                 // the leading (-1, -1) entry
+            info[4] = 0;
+            info[5] = info[6] = info[7] = -1;
+            bf.vel_plan[b] = bf.vel[b];
+        }
+        return;
+    }
     // a scenario whose start pose was rejected (set_startpos returned True, LTPL:268-298) stays so until it is re-anchored
     const int old_flags = bf.sc_flags[b];
     if (old_flags & (LTPL_SC_OUT_OF_TRACK | LTPL_SC_HEADING_MISMATCH)) return;
@@ -235,7 +250,8 @@ k_ref(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm,
     const int B = dm.batch;
     if (bf.sc_flags[b] != 0) return;
     const int* info = bf.st_info + 8 * (size_t)b;
-    if (bf.const_len[b] == 0) {   // OTH:592-598: no valid last solution -> cut 0, no vel_course, vel_plan = v_start (k_state)
+    if (bf.const_len[b] == 0 || info[0] < 0) {   // OTH:592-598: no valid last solution (or a restart) -> cut 0, no
+                                                 // vel_course, vel_plan = v_start (k_state)
         if (lane < LTPL_NSLOT) {
             int* tr = bf.trim + 4 * (size_t)(lane * B + b);
             tr[0] = tr[1] = tr[2] = tr[3] = 0;
@@ -396,7 +412,8 @@ k_backup(const __grid_constant__ LtplParams prm, const __grid_constant__ LtplDim
     if (!(st & LTPL_ST_TRAJ_VALID) || !(st & LTPL_ST_VEL_BOUND_VIOL) ||
         !(act == LTPL_ACT_FOLLOW || act == LTPL_ACT_STRAIGHT))
         return;
-    if (bf.const_len[b] == 0) return;                                  // invalid last solution: no backup plan (OTH:339-344)
+    if (bf.const_len[b] == 0 || bf.st_info[8 * (size_t)b] < 0) return;   // invalid last solution or restart: no backup
+                                                                         // plan (OTH:339-344)
     const int pa = bf.prev_action_id[q];
     if (!(pa == LTPL_ACT_FOLLOW || pa == LTPL_ACT_STRAIGHT)) return;   // no backup plan: stays flagged
     const int m_b = bf.prev_trim[4 * q + 0], L_b = bf.prev_trim[4 * q + 1];

@@ -845,8 +845,10 @@ k_vel_res(const LatDev lt, const LtplParams prm, const LtplDims dm, const LtplBu
         if (!vel_bound) st |= LTPL_ST_VEL_BOUND_VIOL;
         // stateful tick: a backup plan exists (OTH:325-344), so a straight / follow profile that breaks the bound is
         // replaced by a brake profile on the OLD path (OTH:950-1006): flag here, k_backup plans it and clears the flag (no
-        // backup plan exists after an invalid last solution, const_len == 0: the profile is kept, OTH:945-948)
-        if (STATE && !vel_bound && (action == LTPL_ACT_FOLLOW || action == LTPL_ACT_STRAIGHT) && bf.const_len[b] != 0)
+        // backup plan exists after an invalid last solution, const_len == 0, or a restart, st_info[0] < 0: the profile is
+        // kept, OTH:945-948)
+        if (STATE && !vel_bound && (action == LTPL_ACT_FOLLOW || action == LTPL_ACT_STRAIGHT) && bf.const_len[b] != 0 &&
+            bf.st_info[8 * (size_t)b] >= 0)
             atomicOr(&bf.sc_flags[b], LTPL_SC_STATE_FALLBACK | (6 << LTPL_SC_REASON_SHIFT));
         if (vel_bound || action == LTPL_ACT_FOLLOW || action == LTPL_ACT_STRAIGHT) {
             st |= LTPL_ST_TRAJ_VALID;

@@ -543,13 +543,44 @@ class BatchPlanner(object):
         self.buf.trim = t["trim"].data_ptr()
         self._state = st
 
-    def _stage_next(self, sc: ScenarioBatch, sel_action, t_const, vel_est) -> None:
+    def _restart_mask(self, restart):
+        """the restart mask of a stateful tick as a bool array [B], or None when no scenario restarts"""
+        if restart is None:
+            return None
+        mask = np.asarray(restart)
+        if mask.shape != (self.dims.batch,):
+            raise ValueError("restart must be a boolean array of shape [%d], got shape %s" % (self.dims.batch,
+                                                                                          mask.shape))
+        mask = mask.astype(bool)
+        return mask if mask.any() else None
+
+    def _stage_restart(self, mask) -> None:
+        """buffers.restart: NULL without restarts; else its own small H2D copy (the packed input upload stays as it is)"""
+        if mask is None:
+            self.buf.restart = None
+            return
+        st = self._state
+        if "restart" not in st:
+            st["restart"] = torch.zeros((self.dims.batch,), dtype=torch.int32, device=self.device)
+            st["h_restart"] = torch.zeros((self.dims.batch,), dtype=torch.int32).pin_memory()
+            st["restart_ev"] = None
+        if st["restart_ev"] is not None:      # the last copy may still read the pinned staging
+            st["restart_ev"].synchronize()
+        st["h_restart"].numpy()[...] = mask
+        st["restart"].copy_(st["h_restart"], non_blocking=True)
+        st["restart_ev"] = torch.cuda.Event()
+        st["restart_ev"].record(torch.cuda.current_stream(self.device))
+        self.buf.restart = st["restart"].data_ptr()
+
+    def _stage_next(self, sc: ScenarioBatch, sel_action, t_const, vel_est, restart=None) -> None:
         """host side of a stateful tick: pointer swaps, the host memcpy into the pinned staging set, ONE packed H2D copy
-        (scenario arrays incl. sel_action / t_const) and ONE device copy (the small per-path arrays of the last tick)."""
+        (scenario arrays incl. sel_action / t_const) and ONE device copy (the small per-path arrays of the last tick);
+        with restarts one more small H2D copy (the mask)."""
         if sc.size != self.dims.batch:
             raise ValueError("stateful tick: the batch size must not change within a session (re-anchor with "
-                             "set_startpos on a new batch)")
+                             "set_startpos on a new batch, or restart single scenarios with `restart`)")
         check_object_count(sc.obj.shape[1], self.max_objects)   # before the swaps below: a refused list changes nothing
+        mask = self._restart_mask(restart)                       # (likewise)
         if self._state is None:
             self._alloc_state()
         st, t, buf = self._state, self.t, self.buf
@@ -593,14 +624,18 @@ class BatchPlanner(object):
         if self.on_device_start is not None:   # measurement hook: the host staging ends here, the device work begins
             self.on_device_start()
         self.upload()
+        self._stage_restart(mask)
 
-    def next_calc_paths(self, sc: ScenarioBatch, sel_action, t_const, vel_est=None) -> None:
+    def next_calc_paths(self, sc: ScenarioBatch, sel_action, t_const, vel_est=None, restart=None) -> None:
         """calc_paths of a stateful tick (OTH:289-516 with the iterative memory): ``sc`` carries the object
         lists (its poses are only used by ``next_calc_vel_profile``), ``sel_action`` = action id (capi.ACT_*) every
         scenario executed since the last tick, ``t_const`` = min(average calculation time * calc_time_safety, 0.5) per
         scenario (OTH:353-375; the caller keeps the moving average).  The previous tick (tick() / calc_paths() +
-        calc_vel_profile() after set_startpos(), or a stateful tick) must have run on this planner."""
-        self._stage_next(sc, sel_action, t_const, vel_est)
+        calc_vel_profile() after set_startpos(), or a stateful tick) must have run on this planner.
+        ``restart``: boolean array [B]; a true entry restarts that scenario inside this tick, as set_startpos(sc.pos[b],
+        sc.heading[b], sc.vel[b]) on a live planner followed by a first tick (its memory is dropped, its sel_action and
+        t_const are ignored); the other scenarios keep theirs.  A wrong shape raises ValueError and changes nothing."""
+        self._stage_next(sc, sel_action, t_const, vel_est, restart)
         self._call("ltpl_next_calc_paths_batch")
 
     def next_calc_vel_profile(self, pos_est=None, vel_est=None) -> None:
@@ -610,9 +645,10 @@ class BatchPlanner(object):
             self.set_estimates(pos_est, vel_est)
         self._call_vel("ltpl_next_calc_vel_profile_batch")
 
-    def next_tick(self, sc: ScenarioBatch, sel_action, t_const, vel_est=None) -> None:
-        """One stateful tick for the whole batch in one library call: ``sc.pos`` = position estimates."""
-        self._stage_next(sc, sel_action, t_const, vel_est)   # vel_est travels in the packed upload
+    def next_tick(self, sc: ScenarioBatch, sel_action, t_const, vel_est=None, restart=None) -> None:
+        """One stateful tick for the whole batch in one library call: ``sc.pos`` = position estimates (and the new start
+        poses of the scenarios ``restart`` marks, see next_calc_paths)."""
+        self._stage_next(sc, sel_action, t_const, vel_est, restart)   # vel_est travels in the packed upload
         self._call_vel("ltpl_next_tick_batch")
 
     def launch_count(self) -> int:

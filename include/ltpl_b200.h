@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define LTPL_ABI_VERSION 16
+#define LTPL_ABI_VERSION 17
 
 /* action ids (OTH:14-17 ACTION_ID_MAP) */
 #define LTPL_ACT_NONE (-1)
@@ -57,7 +57,8 @@ extern "C" {
 #define LTPL_SC_HEADING_MISMATCH (1 << 1)  /* OTH:234-240                                                             */
 #define LTPL_SC_CAPACITY         (1 << 2)  /* a fixed-capacity buffer (P0_MAX / P_MAX / H_MAX) would overflow          */
 #define LTPL_SC_STATE_FALLBACK   (1 << 4)  /* stateful tick: the last executed trajectory is not usable as memory       */
-                                           /* (see the reason codes; re-anchor with ltpl_set_startpos_batch)                */
+                                           /* (see the reason codes; re-anchor with ltpl_set_startpos_batch, or restart     */
+                                           /* the scenario alone with buffers.restart)                                      */
 #define LTPL_SC_REASON_SHIFT 8             /* bits 8..10: why STATE_FALLBACK was raised (diagnostic detail):            */
                                            /* 1 the executed action is not in the memory and the last tick was not      */
                                            /*   planned either (an action the last tick merely did not return is        */
@@ -261,6 +262,7 @@ typedef struct LtplBuffers {
     const double* t_const;          /* [B] min(average calculation time * calc_time_safety, 0.5) (OTH:353-375): the host  */
                                     /*     keeps the moving average, so the wall clock is an input                         */
     int32_t* st_info;               /* [B][8] k_state: prev path id, prev m, prev L, constant nodes, #factored edges, e0..e2 */
+                                    /*     (prev path id -1: restarted, planned like a first tick)                         */
     int32_t* trim;                  /* [NSLOT*B][4] m = first memory point, L = first memory node, c = first trajectory   */
                                     /*     point (path-plane indices of THIS tick, OTH:586-598, 705-731), pref = #points    */
                                     /*     of vel_course; set to zero by a first tick                                       */
@@ -279,6 +281,12 @@ typedef struct LtplBuffers {
     /* NULL: the constant params.gg_ax / gg_ay of the tuple form.  Rows are aligned with the path planes.                 */
     const double* gg;               /* [2][NSLOT*B][p_max] planes ax_max, ay_max per path point (without gg_scale)         */
     const double* prev_gg;          /* the previous tick's `gg` (brake on the backup plan, OTH:970-975); NULL: constant     */
+    /* restart of single scenarios inside a stateful tick: Graph_LTPL.set_startpos on a live instance (OTH:161-179, 204:   */
+    /* reinit_iterative_memory).  Read by ltpl_next_calc_paths_batch and ltpl_next_tick_batch only; NULL: no restarts.     */
+    /* A restarted scenario drops its memory and is planned like the first tick after set_startpos from pos / heading /    */
+    /* vel (in-track and heading checks, forced 'straight' constant segment, cut 0, profile from vel, no backup plan); its */
+    /* zone is processed anew.  Trajectory ids keep counting.  t_const and sel_action of the scenario are ignored.         */
+    const int32_t* restart;         /* [B] non-zero: set_startpos for this scenario inside the stateful tick               */
 } LtplBuffers;
 
 /* stand-alone forward/backward ggv velocity profile over dense path arrays (BASELINE.json config 5).                   */

@@ -52,6 +52,22 @@ sel = po.t["action_id"].max(dim=0).values.clamp(min=0).cpu().numpy()
 po.next_tick(sc, sel_action=sel, t_const=0.1)
 r = po.records()
 print("70-object stateful tick, trajectories:", sum(len(x.get("traj", {})) for x in r))
+# restarts inside a stateful tick (masked k_startpos in front of k_state): every third scenario, a few of them to a
+# pose off the track, emergency trajectory on, then a stateful tick without restarts
+sc = make_scenarios(Track(H.TRACK_CSV), n, seed=81, n_obj_min=0, n_obj_max=3)
+pr = BatchPlanner(H.lattice_for("default"), device="cuda:0", stateful=True)
+pr.set_vel_params(ax_max_machines=g["ax_max_machines"], incl_emerg_traj=True, **VEL)
+pr.stage_scenarios(sc); pr.upload(); pr.set_startpos(); pr.tick()
+sel = pr.t["action_id"].max(dim=0).values.clamp(min=0).cpu().numpy()
+mask = np.arange(n) % 3 == 0
+sc2 = make_scenarios(Track(H.TRACK_CSV), n, seed=82, n_obj_min=0, n_obj_max=3)
+sc.pos[mask], sc.heading[mask], sc.vel[mask] = sc2.pos[mask], sc2.heading[mask], sc2.vel[mask]
+sc.pos[:9:3] += 40.0
+pr.next_tick(sc, sel_action=sel, t_const=0.1, restart=mask)
+sel = pr.t["action_id"].max(dim=0).values.clamp(min=0).cpu().numpy()
+pr.next_tick(sc, sel_action=sel, t_const=0.1)
+r = pr.records()
+print("stateful tick after restarts, trajectories:", sum(len(x.get("traj", {})) for x in r))
 mb =make_velocity_microbench(200, 150, seed=3)
 vx, ax = calc_vel_profile_batch(pl, mb["kappa"], mb["el"], mb["v_start"], mb["v_end"])
 print("dense vx mean", float(np.mean(vx)))
