@@ -172,23 +172,6 @@ def zone_of(g, b, tick=0):
                             np.zeros((2, 2))]}
 
 
-def tick_snapshot(pl):
-    """the results of a BatchPlanner's last tick as arrays that are byte-comparable across runs: rows of the compact
-    export are gathered through traj_row (their order is unspecified), entries behind the valid lengths are cleared."""
-    f = pl.fetch("action_id", "status", "n_nodes", "nodes", "path_len", "traj_len", "traj_row", "traj", "em_info",
-                 "sc_flags")
-    ok = f["traj_row"] >= 0
-    rows = np.zeros(f["traj_row"].shape + f["traj"].shape[1:], dtype=np.float32)
-    rows[ok] = f["traj"][f["traj_row"][ok]]
-    rows[np.arange(rows.shape[2])[None, None, :] >= f["traj_len"][..., None]] = 0.0
-    nodes = f["nodes"].copy()
-    nodes[np.arange(nodes.shape[2])[None, None, :] >= f["n_nodes"][..., None]] = -1
-    em = f["em_info"].copy()
-    em_rows = f["traj"][np.maximum(em[:, 0], 0)] * (em[:, 0] >= 0)[:, None, None]
-    return dict(action_id=f["action_id"], status=f["status"], nodes=nodes, path_len=f["path_len"],
-                traj_len=f["traj_len"], rows=rows, em_len=em[:, 1], em_rows=em_rows, flags=f["sc_flags"])
-
-
 def compare_emergency(rec, g, b, ctx=""):
     """'emergency' entry (OTH:1027-1034) of a tick record against the zone / emergency fixture."""
     n = int(g["em_len"][b])
@@ -210,11 +193,73 @@ VARIANTS = {   # oracle/gen_golden.py VARIANTS: online overrides, vehicle parame
 
 
 class _Sub(object):
-    """view of the arrays of one variant inside ticks_variants_default.npz (keys '<variant>__<name>')."""
+    """view of the arrays of one sub-set inside a fixture with sub-sets (keys '<name>__<key>').  upcast: objects and
+    prediction points stored as float32 (they are float32-representable) are handed out as the float64 arrays the
+    reference was given."""
 
-    def __init__(self, g, name):
-        self.g, self.p = g, name + "__"
+    def __init__(self, g, name, upcast=False):
+        self.g, self.p, self.upcast = g, name + "__", upcast
         self.files = [k[len(self.p):] for k in g.files if k.startswith(self.p)]
 
     def __getitem__(self, k):
-        return self.g[self.p + k]
+        v = self.g[self.p + k]
+        return v.astype(np.float64) if self.upcast and k in ("sc_obj", "sc_pred") else v
+
+
+VA_COLS, VA_IDX = ("vx", "ax"), (5, 6)   # the columns the first-tick feature fixtures hold, and where a (P, 7) row has them
+N_EXPORT = 115                           # exported rows per trajectory
+
+
+def compare_first_tick(rec, g, b, ctx, exported=False, emergency=False):
+    """a tick record (oracle tick() or BatchPlanner.records()) against scenario b of a first-tick fixture that holds the
+    columns vx, ax of every whole profile (ticks_predlong / ticks_manyobj / ticks_smooth.npz; g: a _Sub): action sets,
+    node sequences, reduced-horizon flags and path lengths, where the fixture has them start nodes, closest objects and
+    node indices, trajectory lengths and ids exact, the rest at the tolerances above.  exported: also the exported fp32
+    rows (rec['traj']); emergency: also the emergency trajectory (taken from the exported rows if exported).  Returns the
+    number of compared trajectories."""
+    ctx = "%s scenario %d" % (ctx, b)
+    assert bool(rec["out_of_track"]) == bool(g["out_of_track"][b]), ctx + " out_of_track"
+    if rec["out_of_track"]:
+        return 0
+    if "start_node" in g.files:
+        assert list(rec["start_node"]) == g["start_node"][b].tolist(), ctx + " start node"
+        coi = -1 if rec["closest_obj_index"] is None else int(rec["closest_obj_index"])
+        assert coi == int(g["closest_obj_index"][b]), ctx + " closest_obj_index %d vs %d" % (
+            coi, int(g["closest_obj_index"][b]))
+    n_traj = 0
+    for a, act in enumerate(ACTIONS):
+        n_want = int(g["path_len"][b, a])
+        has = act in rec["paths"] and len(rec["paths"][act]) > 0
+        assert has == (n_want > 0), "%s: action %s present=%s, golden len %d" % (ctx, act, has, n_want)
+        if has:
+            nodes = [[-1 if v is None else int(v) for v in p] for p in rec["nodes"][act][0]]
+            want = g["nodes"][b, a, :int(g["nodes_len"][b, a])].tolist()
+            assert nodes == want, "%s: node sequence of %s differs\n got  %s\n want %s" % (ctx, act, nodes, want)
+            if "node_idx" in g.files:
+                ni = np.asarray(rec["node_idx"][act][0]).tolist()
+                assert ni == g["node_idx"][b, a, :len(ni)].tolist(), ctx + " node_idx " + act
+            assert bool(rec["red_len"][act][0]) == bool(g["red_len"][b, a]), ctx + " red_len " + act
+            assert rec["paths"][act][0].shape[0] == n_want, ctx + " path length " + act
+        tl = int(g["traj_len"][b, a])
+        assert (act in rec["traj_full"]) == (tl > 0), "%s: trajectory %s present=%s" % (ctx, act, act in rec["traj_full"])
+        if not tl:
+            continue
+        assert int(rec["ids"][act]) % 10 == int(g["traj_id"][b, a]) % 10, ctx + " traj id " + act
+        full = rec["traj_full"][act][0]
+        assert full.shape[0] == tl, ctx + " rows of " + act
+        assert_close("traj[%s]" % act, full[:, VA_IDX], g["traj"][b, a, :tl], VA_COLS, ctx)
+        if exported:
+            rows = rec["traj"][act][0]
+            assert rows.shape[0] == min(tl, N_EXPORT), ctx + " exported rows of " + act
+            assert_close("export[%s]" % act, rows[:, VA_IDX], g["traj"][b, a, :rows.shape[0]], VA_COLS, ctx)
+        n_traj += 1
+    if emergency:
+        n_em = int(g["em_len"][b])
+        em = (rec["traj"] if exported else rec["traj_full"]).get("emergency")
+        assert (em is not None) == (n_em > 0), "%s: emergency present=%s, golden rows %d" % (ctx, em is not None, n_em)
+        if n_em:
+            assert int(rec["ids"]["emergency"]) % 10 == int(g["em_id"][b]) % 10, ctx + " emergency id"
+            ne = min(n_em, N_EXPORT)
+            assert em[0].shape[0] == (ne if exported else n_em), ctx + " emergency rows"
+            assert_close("traj[emergency]", em[0][:ne, VA_IDX], g["em_traj"][b, :ne], VA_COLS, ctx, w_rel=W_REL_BRAKE)
+    return n_traj

@@ -2,6 +2,7 @@
 import numpy as np
 import pytest
 
+from tests import drivers as D
 from tests import helpers as H
 
 pytestmark = pytest.mark.gpu
@@ -13,18 +14,13 @@ def _oracle(tag):
     return OracleLTPL(H.lattice_for(tag))
 
 
-def _planner(tag):
-    from graphbasedlocaltrajectoryplanner_b200.planner import BatchPlanner
-    return BatchPlanner(H.lattice_for(tag), device="cuda:0")
-
-
 @pytest.mark.parametrize("batch", [1, 7, 33, 257])
 def test_ragged_batch_sizes_and_object_counts(batch):
     """batch sizes that do not fill a CTA / warp group; scenarios with 0..K objects mixed in one batch."""
     from graphbasedlocaltrajectoryplanner_b200.scenarios import Track, make_scenarios
     g = H.golden("ticks_default.npz")
     sc = make_scenarios(Track(H.TRACK_CSV), batch, seed=900 + batch, n_obj_min=0, n_obj_max=5, k_max=5)
-    pl = _planner("default")
+    pl = D.planner(H.lattice_for("default"), None)
     pl.set_vel_params(ax_max_machines=g["ax_max_machines"], **VEL)
     pl.stage_scenarios(sc)
     pl.upload()
@@ -54,7 +50,7 @@ def test_out_of_track_heading_mismatch_and_offtrack_objects():
             'length': 5.0, 'width': 2.5}
     ols = [[], [], [far], [far, near]]
     sc = ScenarioBatch.from_object_lists(pos, heading, [20.0] * 4, ols, k_max=2)
-    pl = _planner("default")
+    pl = D.planner(H.lattice_for("default"), None)
     pl.set_vel_params(**VEL)
     pl.stage_scenarios(sc)
     pl.upload()
@@ -77,7 +73,7 @@ def test_vel_max_below_planned_velocity_is_reported():
     from graphbasedlocaltrajectoryplanner_b200.scenarios import Track, make_scenarios
     sc = make_scenarios(Track(H.TRACK_CSV), 16, seed=5, n_obj_min=1, n_obj_max=2)
     sc.vel[:] = 30.0
-    pl = _planner("l216")
+    pl = D.planner(H.lattice_for("l216"), None)
     pl.set_vel_params(vel_max=20.0, gg_scale=1.0, local_gg=(5.0, 5.0), ax_max_machines=np.atleast_2d([100.0, 5.0]),
                       safety_d=30.0)
     pl.stage_scenarios(sc)
@@ -130,7 +126,7 @@ def test_c_abi_error_convention():
     import ctypes as C
     from graphbasedlocaltrajectoryplanner_b200 import capi
     from graphbasedlocaltrajectoryplanner_b200.scenarios import Track, make_scenarios
-    pl = _planner("l216")
+    pl = D.planner(H.lattice_for("l216"), None)
     pl.set_vel_params(**VEL)
     pl.stage_scenarios(make_scenarios(Track(H.TRACK_CSV), 8, seed=1))
     pl.upload()
@@ -167,14 +163,14 @@ def test_tick_under_cuda_graph_capture_replays_identically():
     from graphbasedlocaltrajectoryplanner_b200.scenarios import Track, make_scenarios
     g = H.golden("ticks_default.npz")
     sc = make_scenarios(Track(H.TRACK_CSV), 300, seed=77, n_obj_min=0, n_obj_max=3)
-    pl = _planner("default")
+    pl = D.planner(H.lattice_for("default"), None)
     pl.set_subbatches(3)
     pl.set_vel_params(ax_max_machines=g["ax_max_machines"], incl_emerg_traj=True, **VEL)
     pl.stage_scenarios(sc)
     pl.upload()
     pl.set_startpos()
     pl.tick()                                   # eager (also the warm-up that sets the kernels' attributes)
-    want = H.tick_snapshot(pl)
+    want = D.tick_snapshot(pl)
     assert (want["traj_len"] > 0).sum() > 300
     side = torch.cuda.Stream()
     side.wait_stream(torch.cuda.current_stream())
@@ -185,7 +181,7 @@ def test_tick_under_cuda_graph_capture_replays_identically():
     for name in ("traj", "traj_row", "traj_len", "action_id", "status"):   # the replay has to produce everything again
         pl.t[name].zero_()
     graph.replay()
-    got = H.tick_snapshot(pl)
+    got = D.tick_snapshot(pl)
     for k in want:
         assert np.array_equal(got[k], want[k]), k
 
@@ -214,7 +210,7 @@ def test_planners_sharing_the_shared_memory_attribute(dev_b):
             if local_gg:
                 pl.set_local_gg_planes(*H.local_gg_planes(pl))
             pl.calc_vel_profile()
-            return H.tick_snapshot(pl)
+            return D.tick_snapshot(pl)
 
     a, b = BatchPlanner(H.lattice_for("open"), device="cuda:0"), BatchPlanner(H.lattice_for("open"), device=dev_b)
     for pl in (a, b):

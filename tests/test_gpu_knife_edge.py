@@ -6,6 +6,7 @@ and open lattices, with 1 and 4 scenario windows."""
 import numpy as np
 import pytest
 
+from tests import drivers as D
 from tests import helpers as H
 from tests import knife_edge as K
 
@@ -15,12 +16,8 @@ SETS = ("default", "l216", "open")
 VEL = dict(vel_max=100.0, gg_scale=1.0, local_gg=(5.0, 5.0), safety_d=30.0)
 
 
-def _planner(lat, windows):
-    from graphbasedlocaltrajectoryplanner_b200.planner import BatchPlanner
-    pl = BatchPlanner(lat, device="cuda:0")
-    pl.set_subbatches(windows)
-    pl.set_vel_params(ax_max_machines=H.golden("ticks_manyobj.npz")["ax_max_machines"], **VEL)
-    return pl
+def _axm():
+    return H.golden("ticks_manyobj.npz")["ax_max_machines"]
 
 
 def _batch(scen):
@@ -70,7 +67,7 @@ def test_ego_decisions_at_the_boundary(tag):
         for h in K.window(g["f3_h"][k, 0]):
             add(pos, h, 0 if K.heading_ok(orc, h, psi) else capi.SC_HEADING_MISMATCH, None, "F3 window %d" % k)
     scen = [(p, 0.0 if h is None else h, o) for p, h, o in scen]
-    pl = _planner(orc.lat, 1)
+    pl = D.planner(orc.lat, 1, ax_max_machines=_axm())
     pl.stage_scenarios(_batch(scen))
     pl.upload()
     pl.set_startpos()
@@ -144,7 +141,7 @@ def test_object_decisions_at_the_boundary(tag, windows):
     orc = K.oracle_for(tag)
     scen, want_co, want_cs, ctx = _object_scenarios(g, orc)
     reps = max(1, -(-2048 // len(scen))) if windows > 1 else 1   # enough scenarios for 4 windows of >= 512
-    pl = _planner(orc.lat, windows)
+    pl = D.planner(orc.lat, windows, ax_max_machines=_axm())
     pl.stage_scenarios(_batch(scen * reps))
     pl.upload()
     pl.set_startpos()
@@ -186,7 +183,7 @@ def test_collision_decisions_at_the_boundary(tag):
         scen.append(K.ego_pose(orc, int(g["f5_ego"][g["f5_eq_case"][k]])) + ([K.obj(p)],))
         want.append(g["f5_eq_obs"][k])
         ctx.append("F5 equality %d" % k)
-    pl = _planner(orc.lat, 4)
+    pl = D.planner(orc.lat, 4, ax_max_machines=_axm())
     pl.stage_scenarios(_batch(scen))
     pl.upload()
     pl.set_startpos()
@@ -231,7 +228,7 @@ def test_constant_segment_decisions_at_the_boundary(tag):
         scen.append((g["f6r_ego"][k], g["f6r_hd"][k], [K.obj(p)]))
         fixed.append(g["f6r_obs"][k])
         ctx.append("F6 race-line near-tie %d (gap %.1e)" % (k, g["f6r_gap"][k]))
-    pl = _planner(orc.lat, 4)
+    pl = D.planner(orc.lat, 4, ax_max_machines=_axm())
     pl.stage_scenarios(_batch(scen))
     pl.upload()
     pl.set_startpos()

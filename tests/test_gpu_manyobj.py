@@ -8,32 +8,14 @@ import ctypes as C
 import numpy as np
 import pytest
 
+from tests import drivers as D
 from tests import helpers as H
-from tests.manyobj_golden import VEL, compare_predlong_record, subset, vel_kwargs
 
 pytestmark = pytest.mark.gpu
 
 
-def _planner(lat, windows=4, stateful=False):
-    from graphbasedlocaltrajectoryplanner_b200.planner import BatchPlanner
-    pl = BatchPlanner(lat, device="cuda:0", stateful=stateful)
-    pl.set_subbatches(windows)
-    pl.set_vel_params(ax_max_machines=vel_kwargs()["ax_max_machines"], **VEL)
-    return pl
-
-
-def _first_tick(pl, sc):
-    pl.stage_scenarios(sc)
-    pl.upload()
-    pl.set_startpos()
-    pl.tick()
-
-
-def _snapshot(pl):
-    """H.tick_snapshot without the emergency entries: these ticks do not compute the emergency trajectory."""
-    snap = H.tick_snapshot(pl)
-    del snap["em_len"], snap["em_rows"]
-    return snap
+def vel_kwargs():
+    return dict(D.VEL, ax_max_machines=H.golden("ticks_manyobj.npz")["ax_max_machines"])
 
 
 def _field(tag, B, n_obj, seed, off_frac=0.4, pred_frac=0.0, k_max=None, ahead=(20.0, 500.0)):
@@ -75,30 +57,26 @@ def _field(tag, B, n_obj, seed, off_frac=0.4, pred_frac=0.0, k_max=None, ahead=(
 def test_many_objects_match_reference_golden(name, windows):
     from graphbasedlocaltrajectoryplanner_b200 import capi
     from graphbasedlocaltrajectoryplanner_b200.scenarios import ScenarioBatch
-    sub = subset(name)
+    sub = H._Sub(H.golden("ticks_manyobj.npz"), name, upcast=True)
     n = sub["sc_pos"].shape[0]
     sc = ScenarioBatch.from_object_lists(sub["sc_pos"], sub["sc_heading"], sub["sc_vel"],
                                          [H.object_list(sub, b) for b in range(n)])
     assert sc.obj.shape[1] > 32
-    pl = _planner(H.lattice_for(str(sub["lattice"])), windows)
-    _first_tick(pl, sc)
+    pl = D.planner(H.lattice_for(str(sub["lattice"])), windows, **vel_kwargs())
+    D.first_tick(pl, sc)
     assert pl.dims.k_obj == sc.obj.shape[1]
     recs = pl.records()
     for b in range(n):
         assert not (recs[b]["flags"] & capi.SC_CAPACITY), "scenario %d flagged" % b
-        compare_predlong_record(recs[b], sub, b, ctx="manyobj gpu " + name, exported=True)
+        H.compare_first_tick(recs[b], sub, b, ctx="manyobj gpu " + name, exported=True)
 
 
 def test_facade_plans_a_40_entry_list(tmp_path):
     """Graph_LTPL with 40 entries: on-track and off-track 'physical' objects and non-'physical' entries, interleaved;
     the facade drops the non-'physical' ones on the host, the device the off-track ones."""
-    from graphbasedlocaltrajectoryplanner_b200.Graph_LTPL import Graph_LTPL
     from oracle.ltpl_oracle import OracleLTPL
     sc = _field("default", 6, 32, seed=7101, off_frac=0.4, pred_frac=0.3)
-    pd = {'globtraj_input_path': H.TRACK_CSV, 'graph_store_path': str(tmp_path / "lattice.npz"),
-          'ltpl_offline_param_path': H.OFFLINE_INI, 'ltpl_online_param_path': H.ONLINE_INI}
-    ltpl = Graph_LTPL(path_dict=pd, visual_mode=False, log_to_file=False, device="cuda:0")
-    ltpl.graph_init()
+    ltpl = D.facade(tmp_path)
     orc = OracleLTPL(H.lattice_for("default"))
     vk = vel_kwargs()
     done = 0
@@ -150,8 +128,8 @@ def test_exact_object_counts_match_oracle(zone, pred):
         rng = np.random.default_rng(seed + 7)
         zones = [{"z%d" % b: make_zone(lat, rng, sc.pos[b])} if b % 2 == 0 else None for b in range(sc.size)]
         sc.set_zones(zones)
-    pl = _planner(lat, 3)
-    _first_tick(pl, sc)
+    pl = D.planner(lat, 3, **vel_kwargs())
+    D.first_tick(pl, sc)
     assert pl.dims.k_obj == 200
     recs = pl.records()
     orc = OracleLTPL(lat)
@@ -172,10 +150,10 @@ def test_short_lists_ignore_the_object_capacity():
     lat = H.lattice_for("default")
     sc = _field("default", 256, np.random.default_rng(7301).integers(0, 17, size=256), seed=7302, pred_frac=0.3,
                 k_max=16)
-    pl = _planner(lat, 4)
-    _first_tick(pl, sc)
+    pl = D.planner(lat, 4, **vel_kwargs())
+    D.first_tick(pl, sc)
     assert pl.dims.k_obj == 16
-    plain = _snapshot(pl)
+    plain = D.tick_snapshot(pl, emergency=False)
     big = _field("default", 256, 200, seed=7303, pred_frac=0.3)
     sc2 = sc.subset(np.arange(sc.size))
     K = 200
@@ -188,17 +166,13 @@ def test_short_lists_ignore_the_object_capacity():
     odd = np.arange(1, 256, 2)
     for k in ("pos", "heading", "vel", "n_obj", "obj", "n_pred", "pred"):
         getattr(sc2, k)[odd] = getattr(big, k)[odd]
-    pl2 = _planner(lat, 4)
-    _first_tick(pl2, sc2)
+    pl2 = D.planner(lat, 4, **vel_kwargs())
+    D.first_tick(pl2, sc2)
     assert pl2.dims.k_obj == 200
-    wide = _snapshot(pl2)
     even = np.arange(0, 256, 2)
+    plain, wide = D.take(plain, even), D.take(D.tick_snapshot(pl2, emergency=False), even)
     for k in plain:
-        a, b = plain[k], wide[k]
-        if a.ndim >= 2 and a.shape[0] == 3 and a.shape[1] == sc.size:   # [NSLOT][B] ...
-            assert np.array_equal(a[:, even], b[:, even]), k
-        else:
-            assert np.array_equal(a[even], b[even]), k
+        assert np.array_equal(plain[k], wide[k]), k
 
 
 def test_full_batch_many_objects_invariance():
@@ -208,46 +182,10 @@ def test_full_batch_many_objects_invariance():
     lat = H.lattice_for("l216")
     B = 10000
     sc = _field("l216", B, 48, seed=7401, pred_frac=0.2)
-    pl = _planner(lat, 4)
-    _first_tick(pl, sc)
-    ref = _snapshot(pl)
-
-    def cols(snap, idx):   # scenario-major view of a snapshot restricted to scenarios idx
-        return {k: (v[:, idx] if (v.ndim >= 2 and v.shape[0] == 3 and v.shape[1] == B) else v[idx]) for k, v in snap.items()}
-
-    for windows in (1, 3):
-        pw = _planner(lat, windows)
-        _first_tick(pw, sc)
-        got = _snapshot(pw)
-        for k in ref:
-            assert np.array_equal(ref[k], got[k]), "'%s' differs between 4 and %d scenario windows" % (k, windows)
-    perm = np.random.default_rng(7402).permutation(B)
-    pp = _planner(lat, 4)
-    _first_tick(pp, sc.subset(perm))
-    got = _snapshot(pp)
-    inv = np.argsort(perm)
-    for k in ref:
-        g = got[k]
-        g = g[:, inv] if (g.ndim >= 2 and g.shape[0] == 3 and g.shape[1] == B) else g[inv]
-        assert np.array_equal(ref[k], g), "'%s' depends on the order of the batch" % k
-    part = np.arange(3000, 3700)
-    ps_ = _planner(lat, 2)
-    _first_tick(ps_, sc.subset(part))
-    got, want = _snapshot(ps_), cols(ref, part)
-    for k in want:
-        assert np.array_equal(want[k], got[k]), "'%s' differs in a sub-batch" % k
+    pl = D.assert_batch_invariance(lat, sc, np.random.default_rng(7402).permutation(B), np.arange(3000, 3700),
+                                   **vel_kwargs())
     pick = np.sort(np.random.default_rng(7403).choice(B, size=48, replace=False))
-    recs = pl.records(indices=pick.tolist())
-    orc = OracleLTPL(lat)
-    vk = vel_kwargs()
-    fails = []
-    for rec, b in zip(recs, pick):
-        want = orc.tick(sc.pos[b], sc.heading[b], sc.vel[b], sc.object_list(int(b)), vk)
-        try:
-            H.compare_records(rec, want, ctx="l216 48-object scenario %d" % b)
-        except AssertionError as e:
-            fails.append(str(e).split("\n")[0][:300])
-    assert not fails, "%d/48 sampled scenarios differ from the oracle:\n%s" % (len(fails), "\n".join(fails[:8]))
+    D.assert_sample_matches_oracle(pl, OracleLTPL(lat), sc, pick, vel_kwargs(), "l216 48-object")
 
 
 def test_object_count_beyond_the_bound_is_refused():
@@ -256,10 +194,10 @@ def test_object_count_beyond_the_bound_is_refused():
     from graphbasedlocaltrajectoryplanner_b200 import capi
     from oracle.ltpl_oracle import OracleLTPL
     lat = H.lattice_for("default")
-    pl = _planner(lat, 2)
+    pl = D.planner(lat, 2, **vel_kwargs())
     sc = _field("default", 32, 20, seed=7501)
-    _first_tick(pl, sc)
-    before = _snapshot(pl)
+    D.first_tick(pl, sc)
+    before = D.tick_snapshot(pl, emergency=False)
     bound = pl.max_objects
     assert bound == int(pl.lib.ltpl_max_objects(C.byref(pl.header), int(pl.dims.h_max))) and bound >= 500
     k_keep = pl.dims.k_obj
@@ -271,8 +209,8 @@ def test_object_count_beyond_the_bound_is_refused():
         assert b"too many object slots" in pl.lib.ltpl_last_error(), pl.lib.ltpl_last_error()
     assert pl.launch_count() == n0
     pl.dims.k_obj = k_keep
-    _first_tick(pl, sc)
-    assert all(np.array_equal(before[k], v) for k, v in _snapshot(pl).items())
+    D.first_tick(pl, sc)
+    assert all(np.array_equal(before[k], v) for k, v in D.tick_snapshot(pl, emergency=False).items())
     recs = pl.records(indices=list(range(8)))
     orc = OracleLTPL(lat)
     for b, rec in enumerate(recs):
@@ -288,100 +226,12 @@ def test_closed_loop_many_objects_match_session_oracle():
     """64 sequences x 8 stateful ticks on the default lattice with 20-40 moving objects each (on and off the track, a
     quarter with prediction arrays); the stateful oracle replays the same inputs."""
     from graphbasedlocaltrajectoryplanner_b200 import capi
-    from graphbasedlocaltrajectoryplanner_b200.scenarios import ScenarioBatch
-    from oracle.gen_golden import advance_on_traj
-    from oracle.ltpl_oracle import OracleLTPL
-    from oracle.ltpl_session import OracleSession
     lat = H.lattice_for("default")
     n_seq, n_ticks = 64, 8
     rng = np.random.default_rng(7602)
     sc0 = _field("default", n_seq, rng.integers(20, 41, size=n_seq), seed=7601, pred_frac=0.25, k_max=40)
     prefer = (("right", "left", "straight", "follow"), ("follow", "straight", "left", "right"))
-    pl = _planner(lat, 3, stateful=True)
-
-    class Clk(object):
-        def __init__(self):
-            self.t = 50.0
-
-        def __call__(self):
-            return self.t
-    clks = [Clk() for _ in range(n_seq)]
-    ses = [OracleSession(OracleLTPL(lat), clock=clks[q]) for q in range(n_seq)]
-    objs = sc0.obj.copy()
-    pos_est, vel_est = sc0.pos.copy(), sc0.vel.copy()
-    sel = ["straight"] * n_seq
-    cbuf = [[] for _ in range(n_seq)]
-    alive = np.ones(n_seq, dtype=bool)
-    last_traj = [None] * n_seq
-    vel = vel_kwargs()
-    fails, ticks_ok = [], 0
-    for k in range(n_ticks):
-        dts = rng.uniform(0.04, 0.16, size=n_seq)
-        tcs = np.zeros(n_seq)
-        for q in range(n_seq):
-            dt = float(dts[q])
-            clks[q].t += dt
-            m = int(sc0.n_obj[q])
-            objs[q, :m, 0] -= np.sin(objs[q, :m, 2]) * objs[q, :m, 3] * dt
-            objs[q, :m, 1] += np.cos(objs[q, :m, 2]) * objs[q, :m, 3] * dt
-            if k > 0:
-                if last_traj[q] is not None:
-                    pos_est[q], vel_est[q] = advance_on_traj(last_traj[q], dt)
-                if len(cbuf[q]) >= 5:
-                    cbuf[q].pop(0)
-                cbuf[q].append(dt)
-                tcs[q] = min(float(np.sum(cbuf[q]) / len(cbuf[q])) * 2.0, 0.5)
-        sc = ScenarioBatch(pos_est.copy(), sc0.heading.copy(), sc0.vel.copy(), sc0.n_obj.copy(), objs.copy(),
-                           pred=sc0.pred, n_pred=sc0.n_pred)
-        if k == 0:
-            pl.stage_scenarios(sc, vel_est=vel_est)
-            pl.upload()
-            pl.set_startpos()
-            pl.tick()
-        else:
-            pl.next_tick(sc, sel_action=[H.ACTIONS.index(a) for a in sel], t_const=tcs, vel_est=vel_est)
-        recs = pl.records()
-        for q in range(n_seq):
-            if not alive[q]:
-                continue
-            rec = recs[q]
-            ctx = "sequence %d tick %d (sel %s)" % (q, k, sel[q])
-            if rec["out_of_track"] or (rec["flags"] & (capi.SC_STATE_FALLBACK | capi.SC_BRAKE_PREFIX)):
-                alive[q] = False
-                continue
-            try:
-                if k == 0:
-                    assert ses[q].set_startpos(sc.pos[q], sc.heading[q], sc.vel[q]) is False
-                paths = ses[q].calc_paths(sel[q], sc.object_list(q))
-                traj, _ = ses[q].calc_vel_profile(sc.pos[q], float(vel_est[q]), **vel)
-            except Exception:   # noqa: BLE001  (e.g. the reference's own brake-prefix failure)
-                alive[q] = False
-                continue
-            try:
-                assert not (rec["flags"] & capi.SC_CAPACITY), ctx + " flagged"
-                assert sorted(rec["paths"]) == sorted(paths), "%s: paths %s vs %s" % (ctx, sorted(rec["paths"]),
-                                                                                   sorted(paths))
-                for act in paths:
-                    if ses[q].tie.get(act) or rec["tie"].get(act):
-                        continue
-                    nd = [[-1 if v is None else int(v) for v in p] for p in rec["nodes"][act][0]]
-                    want = [[-1 if v is None else int(v) for v in p] for p in ses[q].m_nodes[act][0]] \
-                        if act in ses[q].m_nodes else None
-                    assert want is None or nd == want, "%s: nodes of %s" % (ctx, act)
-                assert sorted(rec["traj"]) == sorted(traj), ctx + " trajectory set"
-                for act in traj:
-                    H.assert_close("traj[%s]" % act, rec["traj"][act][0], traj[act][0],
-                                   ("s", "x", "y", "psi", "kappa", "vx", "ax"), ctx)
-                ticks_ok += 1
-            except AssertionError as e:
-                fails.append(str(e).split("\n")[0][:400])
-                alive[q] = False
-                continue
-            cand = [a for a in prefer[(q + k) % len(prefer)] if a in rec["traj"]]
-            if not cand:
-                alive[q] = False
-                continue
-            sel[q] = cand[0]
-            last_traj[q] = rec["traj"][sel[q]][0]
-    assert not fails, "%d sequences diverged (%d ticks matched):\n%s" % (len(fails), ticks_ok, "\n".join(fails[:8]))
-    assert ticks_ok > n_seq * n_ticks // 2, ticks_ok
+    n = D.closed_loop_vs_session(D.planner(lat, 3, stateful=True, **vel_kwargs()), lat, sc0, rng, vel_kwargs(), prefer,
+                                 capi.SC_STATE_FALLBACK | capi.SC_BRAKE_PREFIX, n_ticks=n_ticks)
+    assert n["capacity"] == 0, "%d compared ticks flagged SC_CAPACITY" % n["capacity"]
+    assert n["ticks"] > n_seq * n_ticks // 2, n

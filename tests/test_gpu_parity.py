@@ -5,6 +5,7 @@ Node sequences bit-exact; coordinates / velocities within 1e-4 relative (absolut
 import numpy as np
 import pytest
 
+from tests import drivers as D
 from tests import helpers as H
 
 pytestmark = pytest.mark.gpu
@@ -12,14 +13,8 @@ pytestmark = pytest.mark.gpu
 VEL = dict(vel_max=100.0, gg_scale=1.0, local_gg=(5.0, 5.0), safety_d=30.0)
 
 
-SUBBATCHES = {"default": 3, "l216": 4, "l430": 1, "open": 5, "layers14": 2}   # scenario windows inside the library
-
-
-def _planner(tag):
-    from graphbasedlocaltrajectoryplanner_b200.planner import BatchPlanner
-    pl = BatchPlanner(H.lattice_for(tag), device="cuda:0")
-    pl.set_subbatches(SUBBATCHES[tag])   # explicit: also for these small batches (uneven windows incl.)
-    return pl
+# scenario windows inside the library, set explicitly also for these small batches (uneven windows incl.)
+SUBBATCHES = {"default": 3, "l216": 4, "l430": 1, "open": 5, "layers14": 2}
 
 
 def _run_batch(pl, sc, axm):
@@ -47,7 +42,7 @@ def test_cuda_matches_reference_golden(tag):
     from graphbasedlocaltrajectoryplanner_b200.scenarios import ScenarioBatch
     g = H.golden("ticks_%s.npz" % tag)
     sc = ScenarioBatch(g["sc_pos"], g["sc_heading"], g["sc_vel"], g["sc_n_obj"], g["sc_obj"])
-    recs = _run_batch(_planner(tag), sc, g["ax_max_machines"])
+    recs = _run_batch(D.planner(H.lattice_for(tag), SUBBATCHES[tag]), sc, g["ax_max_machines"])
     fails = _collect(lambda b: H.compare_record(recs[b], g, b, ctx=tag), sc.size)
     assert not fails, "%d/%d scenarios differ from the reference golden vectors:\n%s" % (
         len(fails), sc.size, "\n".join(fails[:10]))
@@ -58,7 +53,7 @@ def test_cuda_config1_min_example():
     g = H.golden("config1_min_example.npz")
     obj = np.tile(g["obj"][None, None, :], (2, 1, 1))
     sc = ScenarioBatch(g["sc_pos"], g["sc_heading"], g["sc_vel"], np.ones(2, dtype=np.int32), obj)
-    pl = _planner("default")
+    pl = D.planner(H.lattice_for("default"), SUBBATCHES["default"])
     pl.set_vel_params()     # API defaults of calc_vel_profile (LTPL:344-352)
     pl.stage_scenarios(sc)
     pl.upload()
@@ -80,7 +75,7 @@ def test_cuda_matches_oracle_seeded(tag, n, omin, omax):
     track = Track(H.track_csv_for(tag))
     sc = make_scenarios(track, n, seed=4242 + n, n_obj_min=omin, n_obj_max=omax,
                         s_max=(track.length - 8.0) if tag == "open" else None)
-    recs = _run_batch(_planner(tag), sc, axm)
+    recs = _run_batch(D.planner(H.lattice_for(tag), SUBBATCHES[tag]), sc, axm)
     orc = OracleLTPL(H.lattice_for(tag))
     vk = dict(ax_max_machines=axm, **VEL)
 

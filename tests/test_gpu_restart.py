@@ -6,18 +6,10 @@ import functools
 import numpy as np
 import pytest
 
+from tests import drivers as D
 from tests import helpers as H
 
 pytestmark = pytest.mark.gpu
-
-VEL = dict(vel_max=100.0, gg_scale=1.0, local_gg=(5.0, 5.0), safety_d=30.0)
-COLS = ("s", "x", "y", "psi", "kappa", "vx", "ax")
-
-
-@functools.lru_cache(maxsize=None)
-def _lattice(tag):
-    return H.lattice_for(tag)
-
 
 @functools.lru_cache(maxsize=None)
 def _track(tag):
@@ -29,24 +21,9 @@ def _axm():
     return H.golden("ticks_multitick_default.npz")["ax_max_machines"]
 
 
-def _planner(tag, windows=4, online=None, **vel):
-    from graphbasedlocaltrajectoryplanner_b200.planner import BatchPlanner
-    pl = BatchPlanner(_lattice(tag), online=online, device="cuda:0", stateful=True)
-    pl.set_subbatches(windows)
-    pl.set_vel_params(ax_max_machines=_axm(), **dict(VEL, **vel))
-    return pl
-
-
-def _first_tick(pl, sc, vel_est, gg=False):
-    pl.stage_scenarios(sc, vel_est=vel_est)
-    pl.upload()
-    pl.set_startpos()
-    if gg:
-        pl.calc_paths()
-        pl.set_local_gg_planes(*H.local_gg_planes(pl))
-        pl.calc_vel_profile()
-    else:
-        pl.tick()
+def _stateful(tag, windows, online=None, **vel):
+    """a stateful planner on the lattice `tag` (ax_max_machines of the multi-tick fixtures)"""
+    return D.planner(H.lattice_for(tag), windows, stateful=True, online=online, ax_max_machines=_axm(), **vel)
 
 
 def _next_tick(pl, sc, sel, tc, vel_est, restart=None, gg=False):
@@ -66,9 +43,7 @@ def _state(pl):
                  "closest_obj", "cobj", "cobj_start", "path_len", "path", "coeff", "s_vx_ax", "traj", "traj_len",
                  "traj_id", "traj_row", "trim", "em_info", "em_vx")
     st = {k: pl._state[k].cpu().numpy() for k in ("st_info", "vel_plan", "course", "obj_dist", "zone_s0")}
-    rows = np.zeros((NS, B) + f["traj"].shape[1:], dtype=np.float32)
-    ok = f["traj_row"] >= 0
-    rows[ok] = f["traj"][f["traj_row"][ok]]
+    rows = D.export_rows(f)
     em = np.zeros((1, B) + f["traj"].shape[1:], dtype=np.float32)
     emk = f["em_info"][:, 0] >= 0
     em[0, emk] = f["traj"][f["em_info"][emk, 0]]
@@ -144,10 +119,7 @@ class Loop(object):
 
     def take(self, pl):
         f = pl.fetch("action_id", "traj_len", "traj_row", "traj")
-        rows = np.zeros((3, self.sc.size) + f["traj"].shape[1:], dtype=np.float32)
-        ok = f["traj_row"] >= 0
-        rows[ok] = f["traj"][f["traj_row"][ok]]
-        self.rows = (f["action_id"], f["traj_len"], rows)
+        self.rows = (f["action_id"], f["traj_len"], D.export_rows(f))
 
     def restart(self, mask, new_pos, new_heading, new_vel):
         self.pos[mask], self.heading[mask], self.vel[mask] = new_pos, new_heading, new_vel
@@ -182,11 +154,8 @@ def _new_poses(loop, mask, tag, seed, jump_share=0.5):
 def _light(pl):
     """what the session-oracle comparison reads of the last tick (without the large planes)"""
     f = pl.fetch("sc_flags", "action_id", "status", "n_nodes", "nodes", "traj_len", "traj_row", "traj")
-    rows = np.zeros(f["traj_row"].shape + f["traj"].shape[1:], dtype=np.float32)
-    ok = f["traj_row"] >= 0
-    rows[ok] = f["traj"][f["traj_row"][ok]]
     return dict(sc_flags=f["sc_flags"][None], action_id=f["action_id"], status=f["status"], n_nodes=f["n_nodes"],
-                nodes=f["nodes"], traj_len=f["traj_len"], rows=rows)
+                nodes=f["nodes"], traj_len=f["traj_len"], rows=D.export_rows(f))
 
 
 def _assert_scenarios_equal(got, want, idx, ctx, id_shift=0, exact=True):
@@ -219,7 +188,7 @@ def _assert_scenarios_equal(got, want, idx, ctx, id_shift=0, exact=True):
                 assert np.array_equal(g_sv, w_sv), c + " s_vx_ax"
                 assert np.array_equal(g_rows, w_rows), c + " exported rows"
             else:
-                H.assert_close("rows", g_rows.astype(np.float64), w_rows.astype(np.float64), COLS, c)
+                H.assert_close("rows", g_rows.astype(np.float64), w_rows.astype(np.float64), D.EXPORT_COLS, c)
 
 
 def _snap_equal(a, b, idx, ctx):
@@ -239,16 +208,16 @@ def test_restart_sequences_match_reference(fixture, tag, windows):
     from graphbasedlocaltrajectoryplanner_b200.scenarios import ScenarioBatch
     g = H.golden(fixture)
     n_seq, n_ticks = g["dt"].shape
-    pl = _planner(tag, windows, incl_emerg_traj=True)
+    pl = _stateful(tag, windows, incl_emerg_traj=True)
     compared, revived = 0, 0
     rejected_last = g["rejected"][:, 0] > 0
     for k in range(n_ticks):
         sc = ScenarioBatch(g["pos"][:, k].copy(), g["heading"][:, k].copy(), g["vel"][:, k].copy(),
                            g["sc_n_obj"].copy(), g["obj"][:, k].copy())
         pl.set_vel_params(ax_max_machines=g["ax_max_machines"], incl_emerg_traj=True,
-                          **dict(VEL, gg_scale=float(g["gg_scale"][:, k].min())))
+                          **dict(D.VEL, gg_scale=float(g["gg_scale"][:, k].min())))
         if k == 0:
-            _first_tick(pl, sc, g["vel_est"][:, k])
+            D.first_tick(pl, sc, g["vel_est"][:, k])
         else:
             _next_tick(pl, sc, g["sel"][:, k], g["t_const"][:, k], g["vel_est"][:, k], restart=g["restart"][:, k] > 0)
         recs = pl.records()
@@ -263,25 +232,11 @@ def test_restart_sequences_match_reference(fixture, tag, windows):
                 continue
             assert rec["flags"] == 0, "%s: flags %d" % (ctx, rec["flags"])
             revived += int(bool(g["restart"][q, k]) and k > 0 and bool(g["rejected"][q, :k].any()))
-            for a, act in enumerate(H.ACTIONS):
-                n_want = int(g["path_len"][q, k, a])
-                assert (act in rec["paths"]) == (n_want > 0), "%s: path %s" % (ctx, act)
-                if n_want and not rec["tie"].get(act):
-                    nd = [[-1 if v is None else int(v) for v in p] for p in rec["nodes"][act][0]]
-                    assert nd == g["nodes"][q, k, a, :int(g["nodes_len"][q, k, a])].tolist(), ctx + " nodes " + act
-                    assert rec["paths"][act][0].shape[0] == n_want, ctx + " path length " + act
-                t_want = int(g["traj_len"][q, k, a])
-                assert (act in rec["traj"]) == (t_want > 0), "%s: trajectory %s" % (ctx, act)
-                if t_want:
+            compared += D.compare_multitick_row(rec, g, q, k, ctx, True)
+            for a, act in enumerate(H.ACTIONS):   # one id counter for the batch: +10 per tick, restarts do not reset it
+                if act in rec["traj"]:
                     assert rec["ids"][act] == 10 * (k + 1) + a, ctx + " id " + act
                     assert rec["ids"][act] % 10 == int(g["traj_id"][q, k, a]) % 10, ctx + " id " + act
-                    H.assert_close("traj[%s]" % act, rec["traj"][act][0], g["traj"][q, k, a, :t_want], COLS, ctx)
-                    compared += 1
-            n_em = min(int(g["em_len"][q, k]), 115)
-            assert ("emergency" in rec["traj"]) == (n_em > 0), ctx + " emergency"
-            if n_em:
-                H.assert_close("traj[emergency]", rec["traj"]["emergency"][0], g["em_traj"][q, k, :n_em], COLS, ctx,
-                               w_rel=H.W_REL_BRAKE)
     assert compared > 120 and revived >= 2, (compared, revived)
 
 
@@ -295,7 +250,7 @@ def _feature_batch(tag, B, feature, seed):
         sc = make_scenarios(_track(tag), B, seed=seed, n_obj_min=1, n_obj_max=3)
     if feature == "zone":
         rng = np.random.default_rng(seed + 5)
-        sc.set_zones([{"zone_%d" % b: make_zone(_lattice(tag), rng, sc.pos[b])} if b % 2 == 0 else None
+        sc.set_zones([{"zone_%d" % b: make_zone(H.lattice_for(tag), rng, sc.pos[b])} if b % 2 == 0 else None
                       for b in range(B)])
     if feature == "pred":
         rng = np.random.default_rng(seed + 6)
@@ -322,9 +277,9 @@ def test_restart_equals_fresh_first_tick(tag, feature, B):
     gg = feature == "local_gg"
     seed = 4100 + 7 * FEATURES.index((tag, feature, B))
     sc0 = _feature_batch(tag, B, feature, seed)
-    pl = _planner(tag, 4, online=online, incl_emerg_traj=True)
+    pl = _stateful(tag, 4, online=online, incl_emerg_traj=True)
     loop = Loop(sc0, seed + 1)
-    _first_tick(pl, loop.batch(), loop.vel_est, gg)
+    D.first_tick(pl, loop.batch(), loop.vel_est, gg)
     loop.take(pl)
     for _ in range(3):
         loop.advance()
@@ -335,8 +290,8 @@ def test_restart_equals_fresh_first_tick(tag, feature, B):
     loop.restart(mask, *_new_poses(loop, mask, tag, seed + 3))
     sc = loop.batch()
     _next_tick(pl, sc, loop.sel, loop.tc, loop.vel_est, restart=mask, gg=gg)
-    fresh = _planner(tag, 4, online=online, incl_emerg_traj=True)
-    _first_tick(fresh, sc, loop.vel_est, gg)
+    fresh = _stateful(tag, 4, online=online, incl_emerg_traj=True)
+    D.first_tick(fresh, sc, loop.vel_est, gg)
     got, want = _state(pl), _state(fresh)
     idx = np.nonzero(mask)[0]
     assert (want["traj_len"][:, idx] > 0).any(axis=0).sum() >= 0.9 * idx.size
@@ -350,10 +305,10 @@ def test_restart_equals_fresh_first_tick(tag, feature, B):
 def _twin_loop(tag, B, seed, n_before=3):
     """two planners with identical histories (first tick + n_before stateful ticks)"""
     sc0 = _feature_batch(tag, B, "plain", seed)
-    a, c = _planner(tag, 4, incl_emerg_traj=True), _planner(tag, 4, incl_emerg_traj=True)
+    a, c = _stateful(tag, 4, incl_emerg_traj=True), _stateful(tag, 4, incl_emerg_traj=True)
     loop = Loop(sc0, seed + 1)
     for pl in (a, c):
-        _first_tick(pl, loop.batch(), loop.vel_est)
+        D.first_tick(pl, loop.batch(), loop.vel_est)
     loop.take(a)
     for _ in range(n_before):
         loop.advance()
@@ -421,8 +376,8 @@ def test_all_zero_mask_is_no_mask_and_all_ones_is_a_new_session():
     loop.restart(ones, *_new_poses(loop, ones, "l216", 5410))
     sc = loop.batch()
     _next_tick(a, sc, loop.sel, loop.tc, loop.vel_est, restart=ones)
-    fresh = _planner("l216", 4, incl_emerg_traj=True)
-    _first_tick(fresh, sc, loop.vel_est)
+    fresh = _stateful("l216", 4, incl_emerg_traj=True)
+    D.first_tick(fresh, sc, loop.vel_est)
     _assert_scenarios_equal(_state(a), _state(fresh), everything, "all-ones mask", id_shift=10 * 5)
 
 
@@ -475,7 +430,7 @@ def _oracle_compare(ses, clk, dt, restart, pose, sel, objects, pos, vel_est, sna
             assert want is None or nodes[s, :nn[s]].tolist() == want, "%s: nodes of %s" % (ctx, act)
         assert (tl[s] > 0) == (act in traj), "%s: trajectory %s" % (ctx, act)
         if tl[s] > 0:
-            H.assert_close("traj[%s]" % act, rows[s, :tl[s]].astype(np.float64), traj[act][0], COLS, ctx)
+            H.assert_close("traj[%s]" % act, rows[s, :tl[s]].astype(np.float64), traj[act][0], D.EXPORT_COLS, ctx)
             n += 1
     return n
 
@@ -493,9 +448,9 @@ def test_flagged_scenarios_plan_again_after_a_restart():
     sc0.pos[off] += 40.0 * np.column_stack((np.cos(sc0.heading[off]), np.sin(sc0.heading[off])))
     sc0.heading[back] = np.arctan2(np.sin(sc0.heading[back] + np.pi), np.cos(sc0.heading[back] + np.pi))
     sc0.vel[fast] = 120.0                                 # > vel_max + 0.1: the first tick reports BRAKE_PREFIX
-    pl = _planner("default", 3)
+    pl = _stateful("default", 3)
     loop = Loop(sc0, 5701)
-    _first_tick(pl, loop.batch(), loop.vel_est)
+    D.first_tick(pl, loop.batch(), loop.vel_est)
     loop.take(pl)
     loop.advance()
     _next_tick(pl, loop.batch(), loop.sel, loop.tc, loop.vel_est)
@@ -513,17 +468,17 @@ def test_flagged_scenarios_plan_again_after_a_restart():
         loop.cbuf[b] = []
     sc = loop.batch()
     _next_tick(pl, sc, loop.sel, loop.tc, loop.vel_est, restart=mask)
-    fresh = _planner("default", 3)
-    _first_tick(fresh, sc, loop.vel_est)
+    fresh = _stateful("default", 3)
+    D.first_tick(fresh, sc, loop.vel_est)
     got = _state(pl)
     ok = np.nonzero(mask & (got["sc_flags"][0] == 0))[0]
     assert ok.size >= 22, got["sc_flags"][0, :24]
     _assert_scenarios_equal(got, _state(fresh), ok, "revived", id_shift=10 * 2)
     # the revived scenarios against the session oracle: the restart tick and four stateful ticks after it
-    lat = _lattice("default")
-    clks = {b: type("Clk", (), {"t": 50.0, "__call__": lambda self: self.t})() for b in ok}
+    lat = H.lattice_for("default")
+    clks = {b: D.Clock(50.0) for b in ok}
     ses = {b: RestartSession(OracleLTPL(lat), clock=clks[b]) for b in ok}
-    vel_kw = dict(VEL, ax_max_machines=_axm())
+    vel_kw = dict(D.VEL, ax_max_machines=_axm())
     compared = 0
     for k in range(5):
         if k > 0:
@@ -551,24 +506,24 @@ def test_restarts_at_scale_window_invariant_and_match_oracle():
     from tests.restart_session import RestartSession
     B, n_ticks = 10000, 8
     sc0 = _feature_batch("l216", B, "plain", 5800)
-    one, four = _planner("l216", 1), _planner("l216", 4)
+    one, four = _stateful("l216", 1), _stateful("l216", 4)
     loop = Loop(sc0, 5801)
     rng = np.random.default_rng(5802)
     masks = [np.zeros(B, dtype=bool)] + [rng.random(B) < 0.02 for _ in range(n_ticks - 1)]
     hit = np.any(masks, axis=0)
     sample = np.concatenate((rng.choice(np.nonzero(hit)[0], 48, replace=False),
                              rng.choice(np.nonzero(~hit)[0], 16, replace=False)))
-    lat = _lattice("l216")
-    clks = {b: type("Clk", (), {"t": 50.0, "__call__": lambda self: self.t})() for b in sample}
+    lat = H.lattice_for("l216")
+    clks = {b: D.Clock(50.0) for b in sample}
     ses = {b: RestartSession(OracleLTPL(lat), clock=clks[b]) for b in sample}
     alive = {b: True for b in sample}
-    vel_kw = dict(VEL, ax_max_machines=_axm())
+    vel_kw = dict(D.VEL, ax_max_machines=_axm())
     compared, restarts_seen = 0, 0
     for k in range(n_ticks):
         if k == 0:
             sc = loop.batch()
             for pl in (one, four):
-                _first_tick(pl, sc, loop.vel_est)
+                D.first_tick(pl, sc, loop.vel_est)
         else:
             loop.advance()
             if masks[k].any():
@@ -576,7 +531,7 @@ def test_restarts_at_scale_window_invariant_and_match_oracle():
             sc = loop.batch()
             for pl in (one, four):
                 _next_tick(pl, sc, loop.sel, loop.tc, loop.vel_est, restart=masks[k])
-        s1, s4 = H.tick_snapshot(one), H.tick_snapshot(four)
+        s1, s4 = D.tick_snapshot(one), D.tick_snapshot(four)
         for name in s1:
             assert np.array_equal(s1[name], s4[name]), "tick %d: %s depends on the scenario windows" % (k, name)
         f = _light(one)

@@ -4,50 +4,40 @@ Graph_LTPL facade with an online ini that sets the window, and on the full 10 00
 import numpy as np
 import pytest
 
+from tests import drivers as D
 from tests import helpers as H
-from tests.smooth_golden import compare_smooth_record
-from tests.test_gpu_multitick import _Rows, _t_const
 
 pytestmark = pytest.mark.gpu
-
-VEL = dict(vel_max=100.0, gg_scale=1.0, local_gg=(5.0, 5.0), safety_d=30.0)
-EXPORT_COLS = ("s", "x", "y", "psi", "kappa", "vx", "ax")
 
 
 @pytest.mark.parametrize("name,windows", [("w3_default", 1), ("w7_default", 3), ("w5_open", 4)])
 def test_smoothed_first_tick_matches_reference_golden(name, windows):
     """node sequences, whole smoothed profiles (f64 planes), the fp32 export rows k_smooth rewrites, and the emergency
     trajectory."""
-    from graphbasedlocaltrajectoryplanner_b200.planner import BatchPlanner
     from graphbasedlocaltrajectoryplanner_b200.scenarios import ScenarioBatch
     g = H.golden("ticks_smooth.npz")
     sub = H._Sub(g, name)
-    w = int(sub["filt_window"])
-    pl = BatchPlanner(H.lattice_for(str(sub["lattice"])), online=dict(filt_window_width=w), device="cuda:0")
-    pl.set_subbatches(windows)
-    pl.set_vel_params(ax_max_machines=g["ax_max_machines"], incl_emerg_traj=True, **VEL)
+    pl = D.planner(H.lattice_for(str(sub["lattice"])), windows, online=dict(filt_window_width=int(sub["filt_window"])),
+                   ax_max_machines=g["ax_max_machines"], incl_emerg_traj=True)
     n = sub["sc_pos"].shape[0]
     sc = ScenarioBatch.from_object_lists(sub["sc_pos"], sub["sc_heading"], sub["sc_vel"],
                                          [H.object_list(sub, b) for b in range(n)], k_max=3)
-    pl.stage_scenarios(sc)
-    pl.upload()
-    pl.set_startpos()
-    pl.tick()
+    D.first_tick(pl, sc)
     recs = pl.records()
-    n_traj = sum(compare_smooth_record(recs[b], sub, b, ctx=name + " gpu", exported=True) for b in range(n))
+    n_traj = sum(H.compare_first_tick(recs[b], sub, b, ctx=name + " gpu", exported=True, emergency=True)
+                 for b in range(n))
     assert n_traj >= n
 
 
 def _replay_multitick(g, windows):
     """the closed-loop sequences of a multi-tick fixture as one batch on a stateful planner at the fixture's window."""
     from graphbasedlocaltrajectoryplanner_b200 import capi
-    from graphbasedlocaltrajectoryplanner_b200.planner import BatchPlanner
     from graphbasedlocaltrajectoryplanner_b200.scenarios import ScenarioBatch
     n_seq, n_ticks = g["dt"].shape
-    pl = BatchPlanner(H.lattice_for("default"), online=dict(filt_window_width=int(g.g["filt_window"])),
-                      device="cuda:0", stateful=True)
-    pl.set_subbatches(windows)
-    tc = np.array([_t_const(g["dt"][q, 1:]) for q in range(n_seq)])
+    pl = D.planner(H.lattice_for("default"), windows, stateful=True,
+                   online=dict(filt_window_width=int(g.g["filt_window"])), ax_max_machines=g["ax_max_machines"],
+                   incl_emerg_traj=True)
+    tc = np.array([D.t_const(g["dt"][q, 1:]) for q in range(n_seq)])
     fails, compared = [], 0
     alive = np.ones(n_seq, dtype=bool)
     for k in range(n_ticks):
@@ -55,12 +45,9 @@ def _replay_multitick(g, windows):
                            g["obj"][:, k].copy())
         assert len(set(g["gg_scale"][:, k].tolist())) == 1
         pl.set_vel_params(ax_max_machines=g["ax_max_machines"], incl_emerg_traj=True,
-                          **dict(VEL, gg_scale=float(g["gg_scale"][0, k])))
+                          **dict(D.VEL, gg_scale=float(g["gg_scale"][0, k])))
         if k == 0:
-            pl.stage_scenarios(sc, vel_est=g["vel_est"][:, k])
-            pl.upload()
-            pl.set_startpos()
-            pl.tick()
+            D.first_tick(pl, sc, vel_est=g["vel_est"][:, k])
         else:
             pl.next_tick(sc, sel_action=g["sel"][:, k], t_const=tc[:, k - 1], vel_est=g["vel_est"][:, k])
         recs = pl.records()
@@ -72,24 +59,7 @@ def _replay_multitick(g, windows):
             try:
                 assert not rec["out_of_track"] and "error" not in rec and not (rec["flags"] & capi.SC_STATE_FALLBACK), \
                     ctx + " flags %d" % rec["flags"]
-                for a, act in enumerate(H.ACTIONS):
-                    n_want = int(g["path_len"][q, k, a])
-                    assert (act in rec["paths"]) == (n_want > 0), ctx + " path " + act
-                    if n_want and not rec["tie"].get(act):
-                        nd = [[-1 if v is None else int(v) for v in p] for p in rec["nodes"][act][0]]
-                        assert nd == g["nodes"][q, k, a, :int(g["nodes_len"][q, k, a])].tolist(), ctx + " nodes " + act
-                    t_want = int(g["traj_len"][q, k, a])
-                    assert (act in rec["traj"]) == (t_want > 0), ctx + " trajectory " + act
-                    if t_want:
-                        assert rec["traj"][act][0].shape[0] == t_want, ctx + " rows " + act
-                        H.assert_close("traj[%s]" % act, rec["traj"][act][0], g["traj"][q, k, a, :t_want], EXPORT_COLS,
-                                       ctx)
-                        compared += 1
-                n_em = min(int(g["em_len"][q, k]), 115)
-                assert ("emergency" in rec["traj"]) == (n_em > 0), ctx + " emergency presence"
-                if n_em:
-                    H.assert_close("traj[emergency]", rec["traj"]["emergency"][0], g["em_traj"][q, k, :n_em],
-                                   EXPORT_COLS, ctx, w_rel=H.W_REL_BRAKE)
+                compared += D.compare_multitick_row(rec, g, q, k, ctx, True)
             except AssertionError as e:
                 fails.append(str(e)[:400])
                 alive[q] = False            # later ticks of this sequence depend on this one
@@ -102,72 +72,28 @@ def _replay_multitick(g, windows):
 def test_smoothed_next_tick_matches_reference_sequences(group, windows):
     """window 5, emergency trajectory on; group 1 (the odd sequences) loses grip from tick 3 on, so the brake on the backup
     plan behind vel_course is smoothed across the seam.  gg_scale is a per-batch parameter: the groups run apart."""
-    g = _Rows(H.golden("ticks_multitick_smooth_default.npz"), np.arange(group, 12, 2))
+    g = D.Rows(H.golden("ticks_multitick_smooth_default.npz"), np.arange(group, 12, 2))
     assert _replay_multitick(g, windows) > 30
 
 
 def test_facade_with_smoothing_ini_replays_reference_sequences(tmp_path):
     """Graph_LTPL reads filt_window_width = 5 from its online ini and replays three recorded sequences."""
-    from graphbasedlocaltrajectoryplanner_b200.Graph_LTPL import Graph_LTPL
     g = H.golden("ticks_multitick_smooth_default.npz")
     txt = open(H.ONLINE_INI).read()
     assert txt.count("filt_window_width=1\n") == 1
     ini = tmp_path / "online_w5.ini"
     ini.write_text(txt.replace("filt_window_width=1\n", "filt_window_width=%d\n" % int(g["filt_window"])))
-    pd = {'globtraj_input_path': H.TRACK_CSV, 'graph_store_path': str(tmp_path / "lattice.npz"),
-          'ltpl_offline_param_path': H.OFFLINE_INI, 'ltpl_online_param_path': str(ini)}
-    ltpl = Graph_LTPL(path_dict=pd, visual_mode=False, log_to_file=False, device="cuda:0")
-    ltpl.graph_init()
-
-    class Clk(object):
-        t = 10.0
-
-        def __call__(self):
-            return self.t
-    clk = Clk()
-    ltpl.clock = clk
-    compared = 0
-    for q in (0, 3, 6):                                    # sequences without the grip drop (one gg_scale per call)
-        assert ltpl.set_startpos(pos_est=g["sc_pos"][q], heading_est=g["sc_heading"][q], vel_est=g["sc_vel"][q]) is False
-        n_obj = int(g["sc_n_obj"][q])
-        for k in range(int(g["n_done"][q])):
-            clk.t += float(g["dt"][q, k])
-            ol = [{'id': j + 1, 'type': 'physical', 'X': float(o[0]), 'Y': float(o[1]), 'theta': float(o[2]),
-                   'v': float(o[3]), 'length': float(o[4]), 'width': 2.5} for j, o in enumerate(g["obj"][q, k, :n_obj])]
-            paths = ltpl.calc_paths(prev_action_id=(H.ACTIONS + ("emergency",))[int(g["sel"][q, k])], object_list=ol)
-            traj, ids, _ = ltpl.calc_vel_profile(pos_est=g["pos_est"][q, k], vel_est=float(g["vel_est"][q, k]),
-                                                 ax_max_machines=g["ax_max_machines"], incl_emerg_traj=True,
-                                                 **dict(VEL, gg_scale=float(g["gg_scale"][q, k])))
-            ctx = "facade sequence %d tick %d" % (q, k)
-            for a, act in enumerate(H.ACTIONS):
-                assert (act in paths) == (int(g["path_len"][q, k, a]) > 0), ctx + " paths " + act
-                t_want = int(g["traj_len"][q, k, a])
-                assert (act in traj) == (t_want > 0), ctx + " trajectories " + act
-                if t_want:
-                    H.assert_close("traj[%s]" % act, traj[act][0], g["traj"][q, k, a, :t_want], EXPORT_COLS, ctx)
-                    compared += 1
-            if int(g["em_len"][q, k]):
-                H.assert_close("traj[emergency]", traj["emergency"][0], g["em_traj"][q, k, :int(g["em_len"][q, k])],
-                               EXPORT_COLS, ctx, w_rel=H.W_REL_BRAKE)
-    assert compared > 20
+    seqs = (0, 3, 6)                                       # sequences without the grip drop (one gg_scale per call)
+    assert D.replay_facade(D.facade(tmp_path, ini), g, seqs, True) > 20
 
 
-def _first_tick(lat, sc, axm, w, windows):
-    from graphbasedlocaltrajectoryplanner_b200.planner import BatchPlanner
-    pl = BatchPlanner(lat, online=dict(filt_window_width=w), device="cuda:0")
-    pl.set_subbatches(windows)
-    pl.set_vel_params(ax_max_machines=axm, incl_emerg_traj=True, **VEL)
-    pl.stage_scenarios(sc)
-    pl.upload()
-    pl.set_startpos()
-    pl.tick()
+def _smoothed_tick(lat, sc, axm, w, windows):
+    pl = D.planner(lat, windows, online=dict(filt_window_width=w), ax_max_machines=axm, incl_emerg_traj=True)
+    D.first_tick(pl, sc)
     f = pl.fetch("status", "path_len", "traj_len", "traj_row", "traj", "s_vx_ax", "em_info")
-    ok = f["traj_row"] >= 0
+    rows = D.export_rows(f, cut=True)                     # behind the export cut: unspecified
     ne = f["traj"].shape[1]
-    rows = np.zeros(ok.shape + (ne, 7), dtype=np.float32)
-    rows[ok] = f["traj"][f["traj_row"][ok]]
-    rows[np.arange(ne)[None, None, :] >= f["traj_len"][..., None]] = 0.0   # behind the export cut: unspecified
-    em = np.zeros((ok.shape[1], ne, 7), dtype=np.float32)
+    em = np.zeros((rows.shape[1], ne, 7), dtype=np.float32)
     has_em = f["em_info"][:, 0] >= 0
     em[has_em] = f["traj"][f["em_info"][has_em, 0]]
     em[np.arange(ne)[None, :] >= f["em_info"][:, 1:2]] = 0.0
@@ -187,12 +113,12 @@ def test_full_batch_smoothing():
     lat = H.lattice_for("l216")
     B, w = 10000, 5
     sc = make_scenarios(Track(H.TRACK_CSV), B, seed=4242, n_obj_min=1, n_obj_max=3)
-    pl, r5 = _first_tick(lat, sc, axm, w, 4)
+    pl, r5 = _smoothed_tick(lat, sc, axm, w, 4)
     for windows in (1, 5):
-        other = _first_tick(lat, sc, axm, w, windows)[1]
+        other = _smoothed_tick(lat, sc, axm, w, windows)[1]
         for k in r5:
             assert np.array_equal(r5[k], other[k]), "'%s' differs between 4 and %d scenario windows" % (k, windows)
-    r1 = _first_tick(lat, sc, axm, 1, 4)[1]
+    r1 = _smoothed_tick(lat, sc, axm, 1, 4)[1]
     for k in ("status", "path_len", "traj_len", "em", "em_len"):
         assert np.array_equal(r5[k], r1[k]), "'%s' depends on the window" % k
     valid = (r5["status"].reshape(-1) & capi.ST_TRAJ_VALID) != 0
@@ -218,28 +144,6 @@ def test_full_batch_smoothing():
             assert np.array_equal(r5["rows"][s_, b, :tl, 5], v5[q, :tl].astype(np.float32))
             assert np.array_equal(r5["rows"][s_, b, :tl, 6], a5[q, :tl].astype(np.float32))
 
-    rng = np.random.default_rng(4243)
-    pick = np.sort(rng.choice(B, size=48, replace=False))
-    recs = pl.records(indices=pick.tolist())
-    orc = OracleLTPL(lat, online=dict(filt_window_width=w))
-    vk = dict(ax_max_machines=axm, incl_emerg_traj=True, **VEL)
-    fails = []
-    for rec, b in zip(recs, pick):
-        want = orc.tick(sc.pos[b], sc.heading[b], sc.vel[b], sc.object_list(int(b)), vk)
-        ctx = "l216 w5 scenario %d of %d" % (b, B)
-        try:
-            em_g = em_w = None
-            if not rec["out_of_track"]:                   # records() lists 'emergency' with the exported rows only
-                em_g = rec["traj"].pop("emergency", None)
-                rec["ids"].pop("emergency", None)
-            if not want["out_of_track"]:
-                em_w = want["traj"].pop("emergency", None)
-                want["traj_full"].pop("emergency", None)
-                want["ids"].pop("emergency", None)
-            H.compare_records(rec, want, ctx=ctx)
-            assert (em_g is None) == (em_w is None), ctx + " emergency presence"
-            if em_w is not None:
-                H.assert_close("traj[emergency]", em_g[0], em_w[0], EXPORT_COLS, ctx, w_rel=H.W_REL_BRAKE)
-        except AssertionError as e:
-            fails.append(str(e).split("\n")[0][:300])
-    assert not fails, "%d/48 sampled scenarios differ from the oracle:\n%s" % (len(fails), "\n".join(fails[:8]))
+    pick = np.sort(np.random.default_rng(4243).choice(B, size=48, replace=False))
+    D.assert_sample_matches_oracle(pl, OracleLTPL(lat, online=dict(filt_window_width=w)), sc, pick,
+                                   dict(D.VEL, ax_max_machines=axm, incl_emerg_traj=True), "l216 w5", emergency=True)

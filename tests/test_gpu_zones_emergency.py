@@ -3,18 +3,10 @@ produced by the unmodified reference (tests/golden/ticks_ext_default.npz) and ag
 import numpy as np
 import pytest
 
+from tests import drivers as D
 from tests import helpers as H
 
 pytestmark = pytest.mark.gpu
-
-
-def _planner(g):
-    from graphbasedlocaltrajectoryplanner_b200.planner import BatchPlanner
-    pl = BatchPlanner(H.lattice_for("default"), device="cuda:0")
-    pl.set_subbatches(3)   # zones, emergency rows and prediction arrays across three scenario windows
-    pl.set_vel_params(vel_max=100.0, gg_scale=1.0, local_gg=(5.0, 5.0), ax_max_machines=g["ax_max_machines"],
-                      safety_d=30.0, incl_emerg_traj=True)
-    return pl
 
 
 def _golden_record(rec, g, b):
@@ -38,7 +30,8 @@ def test_zones_and_emergency_match_reference_golden():
     sc = ScenarioBatch.from_object_lists(g["sc_pos"], g["sc_heading"], g["sc_vel"], ols, k_max=3,
                                          blocked_zones=[H.zone_of(g, b) for b in range(n)])
     assert sc.zones is not None and int((sc.zone_sel >= 0).sum()) == int((g["zone_layers"][:, 0] >= 0).sum())
-    pl = _planner(g)
+    pl = D.planner(H.lattice_for("default"), 3, ax_max_machines=g["ax_max_machines"],   # zones, emergency rows and
+                   incl_emerg_traj=True)                  # prediction arrays across three scenario windows
     pl.stage_scenarios(sc)
     pl.upload()
     pl.set_startpos()
@@ -67,7 +60,8 @@ def test_zones_and_emergency_match_oracle_seeded():
             zones.append({"z%d" % b: make_zone(lat, rng, sc.pos[b])})
     sc.set_zones(zones)
     assert len(sc.zones) < int((sc.zone_sel >= 0).sum())
-    pl = _planner(g)
+    pl = D.planner(H.lattice_for("default"), 3, ax_max_machines=g["ax_max_machines"],   # zones, emergency rows and
+                   incl_emerg_traj=True)                  # prediction arrays across three scenario windows
     pl.stage_scenarios(sc)
     pl.upload()
     pl.set_startpos()
@@ -131,7 +125,8 @@ def test_unpack_batch_matches_records():
     from graphbasedlocaltrajectoryplanner_b200.scenarios import Track, make_scenarios
     import torch
     g = H.golden("ticks_ext_default.npz")
-    pl = _planner(g)
+    pl = D.planner(H.lattice_for("default"), 3, ax_max_machines=g["ax_max_machines"],   # zones, emergency rows and
+                   incl_emerg_traj=True)                  # prediction arrays across three scenario windows
     sc = make_scenarios(Track(H.TRACK_CSV), 96, seed=31, n_obj_min=0, n_obj_max=3)
     pl.stage_scenarios(sc)
     pl.upload()

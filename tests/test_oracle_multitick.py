@@ -1,20 +1,10 @@
 """Stateful (multi-tick) oracle, oracle/ltpl_session.py, against closed-loop sequences of the unmodified reference driven
 with a scripted clock (tests/golden/ticks_multitick_default.npz, oracle/gen_golden.py:multitick_fixture).
 The checker of the stateful tick on the device (tests/test_gpu_multitick.py, DESIGN.md section 11)."""
-import numpy as np
-
-from tests import helpers as H
-
-
-class _Clock(object):
-    def __init__(self):
-        self.t = 1000.0
-
-    def __call__(self):
-        return self.t
-
-
 import pytest
+
+from tests import drivers as D
+from tests import helpers as H
 
 
 @pytest.mark.parametrize("fixture,emerg,tag", [("ticks_multitick_default.npz", False, "default"),
@@ -37,64 +27,6 @@ def test_session_oracle_matches_reference_sequences(fixture, emerg, tag):
     the even sequences replace their blocked zone by another one (new id) at tick 4 (OLI:155-237, GLNT:43-99); eighth:
     the open track, vehicles running towards the end of the race line (reduced horizons, v_end = 0); further: the 400 x 21
     lattice with 5 objects; the PDtan follow controller with friction-ellipse exponent 1.5, other mass / drag / gg."""
-    from oracle.ltpl_oracle import OracleLTPL
-    from oracle.ltpl_session import OracleSession
-    g = H.golden(fixture)
     tag, _, variant = tag.partition(":")
-    lat = H.lattice_for(tag)
-    vk = dict(vel_max=100.0, gg_scale=1.0, local_gg=(5.0, 5.0), ax_max_machines=g["ax_max_machines"], safety_d=30.0,
-              incl_emerg_traj=emerg)
-    orc_kw = {}
-    ggpp = variant == "ggpp"                                # location dependent local_gg (+ grip drop, emergency trajectory)
-    if ggpp:
-        variant = ""
-        vk.pop("local_gg")
-    if variant:                                            # other controller / vehicle / velocity parameters (H.VARIANTS)
-        online, veh, vel, _ = H.VARIANTS[variant]
-        orc_kw = dict(online=online, **veh)
-        vk.update(vel)
-    n_seq, n_ticks = g["dt"].shape
-    compared = 0
-    for q in range(n_seq):
-        if int(g["n_done"][q]) == 0:
-            continue
-        clock = _Clock()
-        ses = OracleSession(OracleLTPL(lat, **orc_kw), clock=clock)
-        assert ses.set_startpos(g["sc_pos"][q], g["sc_heading"][q], g["sc_vel"][q]) is False
-        n_obj = int(g["sc_n_obj"][q])
-        for k in range(int(g["n_done"][q])):
-            ctx = "sequence %d tick %d" % (q, k)
-            clock.t += float(g["dt"][q, k])
-            ol = [{'id': j + 1, 'type': 'physical', 'X': float(o[0]), 'Y': float(o[1]), 'theta': float(o[2]),
-                   'v': float(o[3]), 'length': float(o[4]), 'width': 2.5} for j, o in enumerate(g["obj"][q, k, :n_obj])]
-            sel = (H.ACTIONS + ("emergency",))[int(g["sel"][q, k])]   # 4: OTH:307-309
-            paths = ses.calc_paths(sel, ol, blocked_zones=H.zone_of(g, q, k))
-            for a, act in enumerate(H.ACTIONS):
-                n_want = int(g["path_len"][q, k, a])
-                assert (act in paths) == (n_want > 0), "%s: path %s present=%s, golden %d" % (ctx, act, act in paths,
-                                                                                            n_want)
-                if n_want:
-                    assert paths[act][0].shape[0] == n_want, ctx + " path length " + act
-                    nd = [[-1 if v is None else int(v) for v in p] for p in ses.m_nodes[act][0]]
-                    assert nd == g["nodes"][q, k, a, :int(g["nodes_len"][q, k, a])].tolist(), ctx + " nodes " + act
-            kw = dict(vk, gg_scale=float(g["gg_scale"][q, k]))   # third fixture: grip drop
-            if ggpp:
-                kw["local_gg"] = {a: [H.local_gg_field(p[0][:, 0:2])] for a, p in paths.items()}
-            traj, ids = ses.calc_vel_profile(g["pos_est"][q, k], float(g["vel_est"][q, k]), **kw)
-            for a, act in enumerate(H.ACTIONS):
-                t_want = int(g["traj_len"][q, k, a])
-                assert (act in traj) == (t_want > 0), "%s: trajectory %s present=%s, golden %d" % (ctx, act, act in traj,
-                                                                                                 t_want)
-                if t_want:
-                    # the id base (+10 per calc_vel_profile call, OTH:669) is instance state of the reference
-                    assert ids[act] % 10 == int(g["traj_id"][q, k, a]) % 10, ctx + " id " + act
-                    H.assert_close("traj[%s]" % act, traj[act][0], g["traj"][q, k, a, :t_want],
-                                   ("s", "x", "y", "psi", "kappa", "vx", "ax"), ctx)
-                    compared += 1
-            if emerg:
-                n_em = int(g["em_len"][q, k])
-                assert ("emergency" in traj) == (n_em > 0), ctx + " emergency"
-                if n_em:
-                    H.assert_close("traj[emergency]", traj["emergency"][0], g["em_traj"][q, k, :n_em],
-                                   ("s", "x", "y", "psi", "kappa", "vx", "ax"), ctx)
-    assert compared > (40 if g["dt"].shape[0] < 12 else (80 if g["dt"].shape[0] < 16 else 150))
+    online, veh, vel, _ = H.VARIANTS.get(variant, (None, None, None, None))   # other controller / vehicle / velocity
+    D.replay_session_oracle(fixture, emerg, tag, online=online, veh=veh, vel=vel, ggpp=variant == "ggpp")

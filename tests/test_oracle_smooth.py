@@ -5,9 +5,8 @@ the host, which need no GPU."""
 import numpy as np
 import pytest
 
+from tests import drivers as D
 from tests import helpers as H
-from tests.smooth_golden import compare_smooth_record
-import tests.test_oracle_multitick as OM
 
 SMOOTH_SETS = ("w3_default", "w7_default", "w5_open")
 
@@ -27,16 +26,15 @@ def test_oracle_matches_reference_smoothed_first_ticks(name):
     smoothed = 0
     for b in range(n):
         rec = orc.tick(sub["sc_pos"][b], sub["sc_heading"][b], sub["sc_vel"][b], H.object_list(sub, b), vk)
-        compare_smooth_record(rec, sub, b, ctx=name)
+        H.compare_first_tick(rec, sub, b, ctx=name, emergency=True)
         smoothed += sum(int(t[0].shape[0] >= w) for t in rec.get("traj_full", {}).values())
     assert smoothed >= n
 
 
-def test_oracle_session_matches_reference_smoothed_sequences(monkeypatch):
+def test_oracle_session_matches_reference_smoothed_sequences():
     """closed loop at window 5 with the emergency trajectory; the grip drops on the odd sequences, so the brake profile on
     the backup plan and its vel_course seam are smoothed too, and the next tick's memory holds smoothed values."""
-    monkeypatch.setitem(H.VARIANTS, "smooth_w5", (dict(filt_window_width=5), {}, {}, 0.0))
-    OM.test_session_oracle_matches_reference_sequences("ticks_multitick_smooth_default.npz", True, "default:smooth_w5")
+    D.replay_session_oracle("ticks_multitick_smooth_default.npz", True, "default", online=dict(filt_window_width=5))
 
 
 def test_conv_filt_semantics():

@@ -2,7 +2,7 @@
 on-track ones become the vehicle list in list order), made by running the UNMODIFIED reference on the shims of
 oracle/gen_golden.py.  Writes exactly one file and nothing else under the repository:
 
-  tests/golden/ticks_manyobj.npz   first ticks; sub-sets '<set>__<name>' (read through tests/manyobj_golden.py):
+  tests/golden/ticks_manyobj.npz   first ticks; sub-sets '<set>__<name>' (read through tests/helpers.py):
                                      default  default lattice, 48 scenarios
                                      l216     ~216 x 11 lattice (lat_resolution 1.0, lon_straight_step 12.0), 32
                                      open     last ~400 m of the open track (points past the track end), 32
