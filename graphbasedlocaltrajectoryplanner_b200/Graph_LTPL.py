@@ -267,7 +267,8 @@ class Graph_LTPL(object):
         if rec.get("error", 0) & capi.SC_BRAKE_PREFIX:
             raise ValueError("vel_plan exceeds vel_max: the reference's brake-prefix branch (OTH:747-754) yields arrays "
                              "of mismatching length and raises; not planned")
-        if (rec["flags"] & capi.SC_STATE_FALLBACK) and ((rec["flags"] >> capi.SC_REASON_SHIFT) & 7) == 7:
+        if (rec["flags"] & capi.SC_STATE_FALLBACK) and \
+                (rec["flags"] & capi.SC_REASON_MASK) >> capi.SC_REASON_SHIFT == capi.SC_REASON_LAST_ROW:
             self.__state = None   # the reference raises here as well (np.argmin of an empty array, OTH:570)
             raise ValueError("pos_est lies at the last row of the last trajectory: no velocity course left "
                              "(OTH:558-574); call set_startpos() again")

@@ -25,6 +25,9 @@ ST_FOUND, ST_REDUCED_HORIZON, ST_TIE_AMBIGUOUS, ST_START_BLOCKED = 1, 2, 4, 8
 ST_TRAJ_VALID, ST_VEL_BOUND_VIOL, ST_TOO_CLOSE, ST_CONST_ONLY, ST_RENAMED_STRAIGHT = 16, 32, 64, 128, 256
 SC_OUT_OF_TRACK, SC_HEADING_MISMATCH, SC_CAPACITY, SC_BRAKE_PREFIX, SC_STATE_FALLBACK = 1, 2, 4, 8, 16
 SC_REASON_SHIFT = 8   # bits 8..10 of sc_flags: why SC_STATE_FALLBACK was raised (include/ltpl_b200.h)
+SC_REASON_MASK = 7 << SC_REASON_SHIFT
+SC_REASON_NOT_IN_MEMORY, SC_REASON_SHORT_TRAJ, SC_REASON_FEW_NODES, SC_REASON_PLACEHOLDER = 1, 2, 3, 4
+SC_REASON_CONST_LONG, SC_REASON_NO_BACKUP, SC_REASON_LAST_ROW = 5, 6, 7
 
 PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 CSRC_DIR = os.path.join(PKG_DIR, "csrc")

@@ -20,6 +20,15 @@
 #include "ltpl_state.cuh"
 #include "ltpl_smooth.cuh"
 
+// the memory records are the int32 arrays BatchPlanner allocates: st_info [B][8], trim [NSLOT*B][4]
+static_assert(sizeof(LtplStateInfo) == 8 * sizeof(int32_t) && alignof(LtplStateInfo) == alignof(int32_t), "st_info row");
+static_assert(offsetof(LtplStateInfo, prev_q) == 0 && offsetof(LtplStateInfo, prev_m) == 4 &&
+              offsetof(LtplStateInfo, prev_L) == 8 && offsetof(LtplStateInfo, const_nodes) == 12 &&
+              offsetof(LtplStateInfo, n_factored) == 16 && offsetof(LtplStateInfo, factored_edge) == 20, "st_info row");
+static_assert(sizeof(LtplTrim) == 4 * sizeof(int32_t) && alignof(LtplTrim) == alignof(int32_t), "trim row");
+static_assert(offsetof(LtplTrim, m) == 0 && offsetof(LtplTrim, L) == 4 && offsetof(LtplTrim, cut) == 8 &&
+              offsetof(LtplTrim, pref) == 12, "trim row");
+
 static std::atomic<unsigned long long> g_launches{0};
 
 static thread_local std::string g_err;
@@ -502,7 +511,7 @@ static int run_tick(const LtplLattice* lat, const LtplParams* prm, const LtplDim
     const bool paths = stages & kPaths, vel = stages & kVel, memory = bf->trim != nullptr;
     const size_t B = dm->batch;
     if (int r = reset_counts(bf, paths, st)) return r;
-    if (memory && paths && !stateful && cudaMemsetAsync(bf->trim, 0, sizeof(int) * 4 * LTPL_NSLOT * B, st) != cudaSuccess)
+    if (memory && paths && !stateful && cudaMemsetAsync(bf->trim, 0, sizeof(LtplTrim) * LTPL_NSLOT * B, st) != cudaSuccess)
         return fail("memset(trim) failed");
     if (memory && vel && !prm->incl_emerg_traj && bf->em_info &&
         cudaMemsetAsync(bf->em_info, 0xFF, sizeof(int) * 3 * B, st) != cudaSuccess)

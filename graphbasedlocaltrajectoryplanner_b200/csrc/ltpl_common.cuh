@@ -108,6 +108,62 @@ __device__ __forceinline__ int sub_path(const LtplDims& dm, int warps_per_cta) {
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
+// the iterative memory of a stateful tick as k_state left it (LtplStateInfo, LtplTrim)
+// ---------------------------------------------------------------------------------------------------------------------
+// a valid last solution: neither an executed action the last tick did not return (const_len == 0, OTH:393-407) nor a
+// restart.  Without one the trajectory is cut at 0 with no vel_course, and no backup plan exists (OTH:339-344, 592-598).
+__device__ __forceinline__ bool has_last_solution(const LtplBuffers& bf, int b) {
+    return bf.const_len[b] != 0 && bf.st_info[b].prev_q >= 0;
+}
+
+// first trajectory point of path q: 0 in a first tick and in a planner without memory.  Addressed as the int32 word
+// 4 q + 2 (static_asserts in ltpl_api.cu): the export kernels then compile to the code they had before the type.
+__device__ __forceinline__ int trim_cut(const LtplBuffers& bf, int q) {
+    return bf.trim ? reinterpret_cast<const int32_t*>(bf.trim)[4 * q + 2] : 0;
+}
+
+// where the constant segment of scenario b (of B) and the list entries in front of its start node come from: the memory
+// of the last executed trajectory (from its first memory point m and node L on), or set_startpos's segment in a first
+// tick and in a scenario restarted in this tick.  Fields a caller does not read cost nothing.
+struct ConstView {
+    bool mem;              // from the memory; the pointers below are valid only then
+    const double* seg;     // plane x of the constant segment; plane c (x, y, psi, kappa, el) at seg + c * plane
+    size_t plane;
+    int m;                 // first memory point: the memory's node indices count from it
+    int rows;              // coefficient rows of the memory
+    const int* nodes;      // [][2] memory node list
+    const int* node_idx;   // memory node-index list
+    const double* coeff;   // [][8] memory coefficient rows
+};
+template <bool STATE>
+__device__ __forceinline__ ConstView const_view(const LtplDims& dm, const LtplBuffers& bf, int b, int B) {
+    ConstView v;
+    v.plane = (size_t)B * dm.p0_max;
+    v.seg = bf.const_seg + (size_t)b * dm.p0_max;
+    v.m = v.rows = 0;
+    v.nodes = v.node_idx = nullptr;
+    v.coeff = nullptr;
+    v.mem = STATE && bf.st_info[b].prev_q >= 0;
+    if (v.mem) {
+        const LtplStateInfo& si = bf.st_info[b];
+        const size_t row = (size_t)si.prev_q * dm.h_max + si.prev_L;
+        v.plane = (size_t)LTPL_NSLOT * B * dm.p_max;
+        v.seg = bf.prev_path + (size_t)si.prev_q * dm.p_max + si.prev_m;
+        v.m = si.prev_m;
+        v.rows = bf.prev_n_nodes[si.prev_q] - si.prev_L - 1;
+        v.nodes = bf.prev_nodes + row * 2;
+        v.node_idx = bf.prev_node_idx + row;
+        v.coeff = bf.prev_coeff + row * 8;
+    }
+    return v;
+}
+
+// the memory's constant nodes in front of the start node (OTH:462-466), entries i0, i0 + step, ... of the node list
+__device__ __forceinline__ void copy_const_nodes(const ConstView& v, int cnd, int* nd, int i0, int step) {
+    for (int i = i0; i < 2 * cnd; i += step) nd[i] = v.nodes[i];
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
 // float64 helpers with NumPy operation order
 // ---------------------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ double sq_rn(double a) { return __dmul_rn(a, a); }

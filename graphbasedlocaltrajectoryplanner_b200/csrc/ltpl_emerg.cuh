@@ -41,7 +41,7 @@ k_emergency(const __grid_constant__ LtplParams prm, const __grid_constant__ Ltpl
         }
         return;
     }
-    const int cut = bf.trim ? bf.trim[4 * q + 2] : 0;   // stateful tick: the trajectory starts at the cut index
+    const int cut = trim_cut(bf, q);   // stateful tick: the trajectory starts at the cut index
     const int n = bf.path_len[q] - cut;
     const int ne = min(n, dm.n_export);          // exported rows
     const int m = min(n, ne + 1);                // points the rows depend on (ax of row ne - 1 needs w[ne])

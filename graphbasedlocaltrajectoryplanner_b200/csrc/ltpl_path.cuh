@@ -25,7 +25,7 @@ __device__ __forceinline__ void enqueue_path(const LtplBuffers& bf, const LtplDi
 #define LTPL_PATH_MINB 8
 #endif
 // STATE: stateful tick (ltpl_state.cuh): the constant part and the list prefixes come from the previous tick's buffers,
-// except for a scenario restarted in this tick (st_info[0] < 0): set_startpos's, as in a first tick
+// except for a scenario restarted in this tick (LTPL_STATE_RESTARTED): set_startpos's, as in a first tick (const_view)
 template <bool STATE>
 __global__ void __launch_bounds__(LTPL_WARPS_PER_CTA * 32, LTPL_PATH_MINB)
 k_path(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm,
@@ -57,23 +57,11 @@ k_path(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm
 
     const int p0 = bf.const_len[b];
     const size_t pplane = (size_t)LTPL_NSLOT * B * dm.p_max;
-    size_t cplane = (size_t)B * dm.p0_max;
-    const double* cs = bf.const_seg + (size_t)b * dm.p0_max;
-    int cnd = 1;                       // list entries in front of the start node
-    const int* mem_ni = nullptr;       // memory node index list (trimmed at L) and its offset m
-    const double* mem_cf = nullptr;
-    int mem_m = 0, mem_rows = 0;
-    const bool mem = STATE && bf.st_info[8 * (size_t)b] >= 0;
-    if (mem) {
-        const int* sinfo = bf.st_info + 8 * (size_t)b;
-        cplane = pplane;
-        cs = bf.prev_path + (size_t)sinfo[0] * dm.p_max + sinfo[1];
-        cnd = sinfo[3];
-        mem_m = sinfo[1];
-        mem_ni = bf.prev_node_idx + (size_t)sinfo[0] * dm.h_max + sinfo[2];
-        mem_cf = bf.prev_coeff + ((size_t)sinfo[0] * dm.h_max + sinfo[2]) * 8;
-        mem_rows = bf.prev_n_nodes[sinfo[0]] - sinfo[2] - 1;   // coefficient rows of the memory
-    }
+    const ConstView cv = const_view<STATE>(dm, bf, b, B);
+    const bool mem = STATE && cv.mem;   // a constant in k_path<false>: its code is that of a kernel without memory
+    const double* cs = cv.seg;
+    const size_t cplane = cv.plane;
+    const int cnd = mem ? bf.st_info[b].const_nodes : 1;   // list entries in front of the start node
     double* pp = bf.path + (size_t)q * dm.p_max;
     int* node_idx = bf.node_idx + (size_t)q * H;
     double* coeff = bf.coeff + (size_t)q * H * 8;
@@ -86,8 +74,8 @@ k_path(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm
             for (int c = 0; c < 5; ++c) pp[c * pplane + k] = cs[c * cplane + k];
         if (lane == 0) {
             if (mem) {   // OTH:486-501: memory lists up to and including the start node
-                for (int i = 0; i < cnd; ++i) node_idx[i] = mem_ni[i] - mem_m;
-                for (int i = 0; i < min(cnd + 1, mem_rows) * 8; ++i) coeff[i] = mem_cf[i];
+                for (int i = 0; i < cnd; ++i) node_idx[i] = cv.node_idx[i] - cv.m;
+                for (int i = 0; i < min(cnd + 1, cv.rows) * 8; ++i) coeff[i] = cv.coeff[i];
             } else {
                 node_idx[0] = 0;
                 for (int c = 0; c < 8; ++c) coeff[c] = bf.const_coeff[(size_t)b * 8 + c];
@@ -246,8 +234,8 @@ k_path(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm
     // ---- stitched bookkeeping (OTH:458-472) ----
     for (int i = lane; i <= nseg; i += 32) node_idx[cnd + i] = nidx[i] + loc;
     if (mem) {
-        for (int i = lane; i < cnd; i += 32) node_idx[i] = mem_ni[i] - mem_m;
-        for (int i = lane; i < cnd * 8; i += 32) coeff[i] = mem_cf[i];
+        for (int i = lane; i < cnd; i += 32) node_idx[i] = cv.node_idx[i] - cv.m;
+        for (int i = lane; i < cnd * 8; i += 32) coeff[i] = cv.coeff[i];
     }
     if (!mem && lane < 8) coeff[lane] = bf.const_coeff[(size_t)b * 8 + lane];
     if (lane == 0) {

@@ -652,7 +652,7 @@ __device__ __forceinline__ int act_filter(int acts, int a) { return (acts >> (5 
 #endif
 // STATE: stateful tick (ltpl_state.cuh): start node / constant segment come from k_state, the constant segment lives in
 // the previous tick's path planes, pos_est and the last action id enter the action-set logic, the first edges of the
-// last solution are cheaper.  A scenario restarted in this tick (st_info[0] < 0) is planned like a first tick: its
+// last solution are cheaper.  A scenario restarted in this tick (LTPL_STATE_RESTARTED) is planned like a first tick: its
 // constant segment, start node and [(-1, -1), start] node list are what k_startpos has just produced.
 template <bool ZONE, bool STATE = false, bool DENSE = false>
 __global__ void __launch_bounds__(LTPL_WARPS_PER_CTA * 32, LTPL_PLAN_MINB)
@@ -693,7 +693,7 @@ k_plan(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm
 
     const int start_layer = bf.start_node[2 * b];
     // entries of the node / node-index / coefficient lists in front of the start node
-    const int cnd = STATE ? bf.st_info[8 * (size_t)b + 3] : 1;
+    const int cnd = STATE ? bf.st_info[b].const_nodes : 1;
 
     // ---- OLI.process_object_list (OLI:96-141): drop off-track objects, radius = length / 2, prediction points; the
     // object slots in chunks of 32 ----
@@ -711,24 +711,17 @@ k_plan(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm
     {   // race-line s coordinates for the constant-segment check (MOPG:80-97), one query: lane 0 the start, lane 1 the
         // end of the constant segment, lane 2 + v vehicle v < 30 (the later ones: chunk_objects)
         const int p0 = bf.const_len[b];
-        size_t cplane = (size_t)dm.batch * dm.p0_max;
-        const double* cs = bf.const_seg + (size_t)b * dm.p0_max;
-        const bool mem = STATE && bf.st_info[8 * (size_t)b] >= 0;   // constant segment from the memory
-        if (mem) {
-            const int* sinfo = bf.st_info + 8 * (size_t)b;
-            cplane = (size_t)LTPL_NSLOT * dm.batch * dm.p_max;
-            cs = bf.prev_path + (size_t)sinfo[0] * dm.p_max + sinfo[1];
-        }
+        const ConstView cv = const_view<STATE>(dm, bf, b, dm.batch);
         double qx = 0.0, qy = 0.0;
         bool q_act = false;
         if (p0 >= 2) {
             q_act = lane < 2 + n_veh;
             if (lane == 0) {   // MOPG:80-84: pos_est of the previous calc_vel_profile call; None on the first tick
-                qx = mem ? bf.pos_last[2 * b] : cs[0];
-                qy = mem ? bf.pos_last[2 * b + 1] : cs[cplane];
+                qx = cv.mem ? bf.pos_last[2 * b] : cv.seg[0];
+                qy = cv.mem ? bf.pos_last[2 * b + 1] : cv.seg[cv.plane];
             } else if (lane == 1) {
-                qx = cs[p0 - 1];
-                qy = cs[cplane + p0 - 1];
+                qx = cv.seg[p0 - 1];
+                qy = cv.seg[cv.plane + p0 - 1];
             } else if (q_act) {
                 qx = vr[lane - 2].x;
                 qy = vr[lane - 2].y;
@@ -824,13 +817,7 @@ k_plan(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm
     // (read here: nothing of the constant segment stays live across the disc stage)
     const int start_node = bf.start_node[2 * b + 1];
     const int p0 = bf.const_len[b];
-    size_t cplane = (size_t)B * dm.p0_max;
-    const double* cs = bf.const_seg + (size_t)b * dm.p0_max;
-    if (STATE && bf.st_info[8 * (size_t)b] >= 0) {
-        const int* sinfo = bf.st_info + 8 * (size_t)b;
-        cplane = (size_t)LTPL_NSLOT * B * dm.p_max;
-        cs = bf.prev_path + (size_t)sinfo[0] * dm.p_max + sinfo[1];
-    }
+    const ConstView cv = const_view<STATE>(dm, bf, b, B);
     bool obj_in_const = false, obj_beside = false;
     if (p0 >= 2) {
         const double s_start = ps->s_seg[0], s_end = ps->s_seg[1];
@@ -853,7 +840,8 @@ k_plan(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm
                 const double oref = sq_rn(__dadd_rn(vr[v].r, __ddiv_rn(lt.veh_width, 2.0)));
                 int hit = 0;
                 #pragma unroll 1
-                for (int k = lane; k < p0; k += 32) hit |= (dist2_rn(cs[k], cs[cplane + k], ox, oy) <= oref) ? 1 : 0;
+                for (int k = lane; k < p0; k += 32)
+                    hit |= (dist2_rn(cv.seg[k], cv.seg[cv.plane + k], ox, oy) <= oref) ? 1 : 0;
                 if (__any_sync(LTPL_FULL, hit)) obj_in_const = true;
             }
         }
@@ -888,8 +876,8 @@ k_plan(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm
     if (obj_in_const || obj_beside) {
         n_act = 1;
         acts = act_entry(0, LTPL_ACT_FOLLOW, 0);
-        // last_action_id (MOPG:130): the executed action, 'emergency' already translated by k_state (st_info[0] = its slot)
-        const int pq = STATE ? bf.st_info[8 * (size_t)b] : -1;
+        // last_action_id (MOPG:130): the executed action, 'emergency' already translated by k_state (prev_q = its slot)
+        const int pq = STATE ? bf.st_info[b].prev_q : -1;
         const int last_act = pq >= 0 ? bf.prev_action_id[pq] : LTPL_ACT_STRAIGHT;
         if (!obj_in_const && (last_act == LTPL_ACT_LEFT || last_act == LTPL_ACT_RIGHT)) {   // MOPG:130-133: keep overtaking
             acts |= act_entry(1, last_act, 1);
@@ -941,11 +929,11 @@ k_plan(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm
     c.ff0 = c.ff1 = c.ff2 = 1.0;
     int n_fe = 0;
     if (STATE) {
-        const int* sinfo = bf.st_info + 8 * (size_t)b;
-        n_fe = sinfo[4];
-        c.fe0 = sinfo[5];
-        c.fe1 = sinfo[6];
-        c.fe2 = sinfo[7];
+        const LtplStateInfo& si = bf.st_info[b];
+        n_fe = si.n_factored;
+        c.fe0 = si.factored_edge[0];
+        c.fe1 = si.factored_edge[1];
+        c.fe2 = si.factored_edge[2];
         c.ff0 = prm.w_last_edges[0];
         c.ff1 = prm.w_last_edges[1];
         c.ff2 = prm.w_last_edges[2];
@@ -1056,14 +1044,10 @@ k_plan(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm
             if (src == 1) gj = dp_goal(lt, lane, c, &tie, goal_off);
             if (tie) st |= LTPL_ST_TIE_AMBIGUOUS;
             st |= LTPL_ST_FOUND;
-            const bool mem = STATE && bf.st_info[8 * (size_t)b] >= 0;
-            if (mem && src != 2) {   // constant nodes in front of the start node: the memory of the last tick (OTH:462-466)
-                const int* sinfo = bf.st_info + 8 * (size_t)b;
-                const int* pn = bf.prev_nodes + ((size_t)sinfo[0] * dm.h_max + sinfo[2]) * 2;
-                for (int i = lane; i < 2 * cnd; i += 32) nd[i] = pn[i];
-            }
+            const ConstView cv = const_view<STATE>(dm, bf, b, B);
+            if (cv.mem && src != 2) copy_const_nodes(cv, cnd, nd, lane, 32);
             if (lane == 0) {
-                if (!mem) {
+                if (!cv.mem) {
                     nd[0] = -1;
                     nd[1] = -1;
                 }
@@ -1106,10 +1090,9 @@ k_plan(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm
         if (!any && bf.const_len[b] > 2) {   // (re-read: p0 is not kept live across the searches)
             const int q = b;
             int* nd = bf.nodes + (size_t)q * dm.h_max * 2;
-            if (STATE && bf.st_info[8 * (size_t)b] >= 0) {
-                const int* sinfo = bf.st_info + 8 * (size_t)b;
-                const int* pn = bf.prev_nodes + ((size_t)sinfo[0] * dm.h_max + sinfo[2]) * 2;
-                for (int i = 0; i < 2 * cnd; ++i) nd[i] = pn[i];
+            const ConstView cv = const_view<STATE>(dm, bf, b, B);
+            if (cv.mem) {
+                copy_const_nodes(cv, cnd, nd, 0, 1);
             } else {
                 nd[0] = -1;
                 nd[1] = -1;

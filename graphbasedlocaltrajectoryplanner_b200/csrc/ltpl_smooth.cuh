@@ -26,7 +26,7 @@ k_smooth(const __grid_constant__ LtplDims dm, const __grid_constant__ LtplBuffer
     if (!(bf.status[q] & LTPL_ST_TRAJ_VALID)) return;
     const int B = dm.batch;
     const size_t pplane = (size_t)LTPL_NSLOT * B * dm.p_max;
-    const int cut = bf.trim ? bf.trim[4 * q + 2] : 0;     // stateful tick: the profile starts at the cut index
+    const int cut = trim_cut(bf, q);                      // stateful tick: the profile starts at the cut index
     const int n = bf.path_len[q] - cut;                   // rows of the whole profile
     double* raw = reinterpret_cast<double*>(sm_smem) + (size_t)(threadIdx.x >> 5) * dm.p_max;
     const double* S = bf.s_vx_ax + (size_t)q * dm.p_max;

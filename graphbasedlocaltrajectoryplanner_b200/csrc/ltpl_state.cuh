@@ -1,10 +1,10 @@
 // ltpl_state.cuh -- stateful tick (DESIGN.md section 11): the iterative memory of OnlineTrajectoryHandler
 // on the device.  The memory of the reference (OTH:64-87: __last_action_set_{path_param, node_idx, nodes, coeff},
-// __last_bp_action_set) IS the output of the previous tick: a second LtplBuffers set (prev_*) used ping-pong, plus three
-// integers per path instead of the slicing of OTH:705-731:
-//     m = first memory point   (cut_index_layer, OTH:712)      path-plane index
-//     L = first memory node    (cut_layer,       OTH:586)      node index
-//     c = first trajectory row (cut_index_pos,   OTH:578)      path-plane index;  __last_cut_idx = c - m (OTH:598)
+// __last_bp_action_set) IS the output of the previous tick: a second LtplBuffers set (prev_*) used ping-pong, plus an
+// LtplTrim per path instead of the slicing of OTH:705-731:
+//     m   = cut_index_layer (OTH:712)
+//     L   = cut_layer       (OTH:586)
+//     cut = cut_index_pos   (OTH:578);  __last_cut_idx = cut - m (OTH:598)
 // The exported trajectory ("bp", <= n_export rows because LTPL:401-406 cuts the dict it shares with the handler) is
 // rows 0 .. traj_len-1 of the previous s / vx planes, its x, y are path-plane points c .. c + traj_len - 1.
 //
@@ -59,18 +59,18 @@ k_state(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams pr
     const int b = sub_scenario(dm, LTPL_WARPS_PER_CTA);
     if (b < 0) return;
     const int B = dm.batch;
-    int* info = bf.st_info + 8 * (size_t)b;
+    LtplStateInfo& info = bf.st_info[b];
     if (bf.restart && bf.restart[b]) {
         // set_startpos on the live instance (OTH:161-179, 204): k_startpos has just checked the pose and seeded the forced
-        // 'straight' segment; the memory is dropped.  Marker for the later kernels: st_info[0] = -1 -- the constant
+        // 'straight' segment; the memory is dropped.  Marker for the later kernels: LTPL_STATE_RESTARTED -- the constant
         // segment is set_startpos's, no cost reduction, cut 0 at vel (get_ref_idx without a last trajectory, OTH:592-598),
         // no backup plan.  A rejected pose keeps the flags k_startpos wrote.
         if (lane == 0 && bf.sc_flags[b] == 0) {
-            info[0] = -1;
-            info[1] = info[2] = 0;
-            info[3] = 1;                                 // the leading (-1, -1) entry
-            info[4] = 0;
-            info[5] = info[6] = info[7] = -1;
+            info.prev_q = LTPL_STATE_RESTARTED;
+            info.prev_m = info.prev_L = 0;
+            info.const_nodes = 1;                        // the leading (-1, -1) entry
+            info.n_factored = 0;
+            info.factored_edge[0] = info.factored_edge[1] = info.factored_edge[2] = -1;
             bf.vel_plan[b] = bf.vel[b];
         }
         return;
@@ -110,21 +110,24 @@ k_state(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams pr
             bf.start_node[2 * b] = old_sl;
             bf.start_node[2 * b + 1] = old_sn;
             bf.const_len[b] = 0;
-            info[0] = b;                                 // a valid row; nothing of it is used (cnd = 0, const_len = 0)
-            info[1] = 0;
-            info[2] = 0;
-            info[3] = 0;
-            info[4] = 0;
-            info[5] = info[6] = info[7] = -1;
+            info.prev_q = b;                             // a valid row; nothing of it is used (cnd = 0, const_len = 0)
+            info.prev_m = 0;
+            info.prev_L = 0;
+            info.const_nodes = 0;
+            info.n_factored = 0;
+            info.factored_edge[0] = info.factored_edge[1] = info.factored_edge[2] = -1;
             bf.vel_plan[b] = bf.vel[b];                  // `vel` of a stateful tick = v_start of set_startpos (OTH:597)
         }
         return;
     }
     if (qp < 0 || nb_rows <= 2) {   // OTH:319-322, constant segment exists but <= 2 trajectory rows: not planned
-        if (lane == 0) bf.sc_flags[b] = LTPL_SC_STATE_FALLBACK | ((qp < 0 ? 1 : 2) << LTPL_SC_REASON_SHIFT);
+        if (lane == 0)
+            bf.sc_flags[b] = LTPL_SC_STATE_FALLBACK |
+                             ((qp < 0 ? LTPL_SC_REASON_NOT_IN_MEMORY : LTPL_SC_REASON_SHORT_TRAJ) << LTPL_SC_REASON_SHIFT);
         return;
     }
-    const int m_p = bf.prev_trim[4 * qp + 0], L_p = bf.prev_trim[4 * qp + 1], c_p = bf.prev_trim[4 * qp + 2];
+    const LtplTrim& tp = bf.prev_trim[qp];
+    const int m_p = tp.m, L_p = tp.L, c_p = tp.cut;
     const size_t pplane = (size_t)LTPL_NSLOT * B * dm.p_max;
     const double* Px = bf.prev_path + (size_t)qp * dm.p_max;
     const double* Py = Px + pplane;
@@ -154,7 +157,7 @@ k_state(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams pr
     // first node after the predicted position (OTH:381-386)
     const int nn_mem = bf.prev_n_nodes[qp] - L_p;   // nodes of the (trimmed) memory
     if (nn_mem < 2) {
-        if (lane == 0) bf.sc_flags[b] = LTPL_SC_STATE_FALLBACK | (3 << LTPL_SC_REASON_SHIFT);
+        if (lane == 0) bf.sc_flags[b] = LTPL_SC_STATE_FALLBACK | (LTPL_SC_REASON_FEW_NODES << LTPL_SC_REASON_SHIFT);
         return;
     }
     const int* Ip = bf.prev_node_idx + (size_t)qp * dm.h_max + L_p;
@@ -165,7 +168,9 @@ k_state(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams pr
     const int loc = Ip[sni] - m_p;                   // loc_path_start_idx within the memory path
     const int sl = Np[2 * sni], sn = Np[2 * sni + 1];
     if (sl < 0 || loc + 1 > dm.p_max) {
-        if (lane == 0) bf.sc_flags[b] = LTPL_SC_STATE_FALLBACK | ((sl < 0 ? 4 : 5) << LTPL_SC_REASON_SHIFT);
+        if (lane == 0)
+            bf.sc_flags[b] = LTPL_SC_STATE_FALLBACK |
+                             ((sl < 0 ? LTPL_SC_REASON_PLACEHOLDER : LTPL_SC_REASON_CONST_LONG) << LTPL_SC_REASON_SHIFT);
         return;
     }
     if (lane == 0) {
@@ -173,22 +178,21 @@ k_state(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams pr
         bf.start_node[2 * b] = sl;
         bf.start_node[2 * b + 1] = sn;
         bf.const_len[b] = loc + 1;
-        info[0] = qp;
-        info[1] = m_p;
-        info[2] = L_p;
-        info[3] = sni;                               // number of constant nodes in front of the start node
+        info.prev_q = qp;
+        info.prev_m = m_p;
+        info.prev_L = L_p;
+        info.const_nodes = sni;
         // cost reduction on the first edges of the remaining last solution (GLNT:155-162)
         int n_fe = 0;
         for (int i = 0; i < 3; ++i) {
-            info[5 + i] = -1;
+            info.factored_edge[i] = -1;
             if (sni + i + 1 < nn_mem) {
-                const int e = find_edge(lt, Np[2 * (sni + i)], Np[2 * (sni + i) + 1], Np[2 * (sni + i + 1)],
-                                        Np[2 * (sni + i + 1) + 1]);
-                info[5 + i] = e;   // slot i keeps factor w_last_edges[i]; -1: edge not in the lattice
+                info.factored_edge[i] = find_edge(lt, Np[2 * (sni + i)], Np[2 * (sni + i) + 1], Np[2 * (sni + i + 1)],
+                                                  Np[2 * (sni + i + 1) + 1]);
                 n_fe = i + 1;
             }
         }
-        info[4] = n_fe;
+        info.n_factored = n_fe;
     }
 }
 
@@ -249,19 +253,17 @@ k_ref(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm,
     if (b < 0) return;
     const int B = dm.batch;
     if (bf.sc_flags[b] != 0) return;
-    const int* info = bf.st_info + 8 * (size_t)b;
-    if (bf.const_len[b] == 0 || info[0] < 0) {   // OTH:592-598: no valid last solution (or a restart) -> cut 0, no
-                                                 // vel_course, vel_plan = v_start (k_state)
+    if (!has_last_solution(bf, b)) {   // OTH:592-598: cut 0, no vel_course, vel_plan = v_start (k_state)
         if (lane < LTPL_NSLOT) {
-            int* tr = bf.trim + 4 * (size_t)(lane * B + b);
-            tr[0] = tr[1] = tr[2] = tr[3] = 0;
+            LtplTrim& tr = bf.trim[lane * B + b];
+            tr.m = tr.L = tr.cut = tr.pref = 0;
         }
         __syncwarp();
         ref_obj_dist(dm, bf, b, 0, bf.pos[2 * b], bf.pos[2 * b + 1], lane);
         return;
     }
-    const int qp = info[0], m_p = info[1];
-    const int c_p = bf.prev_trim[4 * qp + 2];
+    const int qp = bf.st_info[b].prev_q, m_p = bf.st_info[b].prev_m;
+    const int c_p = bf.prev_trim[qp].cut;
     const int nb_rows = bf.prev_traj_len[qp];
     const size_t pplane = (size_t)LTPL_NSLOT * B * dm.p_max;
     const double* Px = bf.prev_path + (size_t)qp * dm.p_max + c_p;   // trajectory row j -> path point c + j
@@ -313,7 +315,7 @@ k_ref(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm,
     }
     vel_idx = __shfl_sync(LTPL_FULL, vel_idx, 0);
     if (vel_idx < 0) {   // np.argmin of an empty array raises in the reference (OTH:570): not planned, re-anchor
-        if (lane == 0) bf.sc_flags[b] = LTPL_SC_STATE_FALLBACK | (7 << LTPL_SC_REASON_SHIFT);
+        if (lane == 0) bf.sc_flags[b] = LTPL_SC_STATE_FALLBACK | (LTPL_SC_REASON_LAST_ROW << LTPL_SC_REASON_SHIFT);
         return;
     }
     const int cut_pos = (c_p - m_p) + cut_index;     // cut_index_pos in the NEW path planes (OTH:577)
@@ -336,14 +338,14 @@ k_ref(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm,
     }
     if (lane < LTPL_NSLOT) {
         const int q = lane * B + b;
-        int* tr = bf.trim + 4 * (size_t)q;
+        LtplTrim& tr = bf.trim[q];
         if (bf.action_id[q] != LTPL_ACT_NONE) {
-            tr[0] = bf.node_idx[(size_t)q * dm.h_max + cut_layer];
-            tr[1] = cut_layer;
-            tr[2] = cut_pos;
-            tr[3] = vel_idx;
+            tr.m = bf.node_idx[(size_t)q * dm.h_max + cut_layer];
+            tr.L = cut_layer;
+            tr.cut = cut_pos;
+            tr.pref = vel_idx;
         } else {
-            tr[0] = tr[1] = tr[2] = tr[3] = 0;
+            tr.m = tr.L = tr.cut = tr.pref = 0;
         }
     }
 
@@ -364,7 +366,7 @@ k_prefix(const __grid_constant__ LtplDims dm, const __grid_constant__ LtplBuffer
     if (q < 0) return;
     if (!(bf.status[q] & LTPL_ST_TRAJ_VALID)) return;
     const int b = q % B;
-    const int cut = bf.trim[4 * q + 2], pref = bf.trim[4 * q + 3];
+    const int cut = bf.trim[q].cut, pref = bf.trim[q].pref;
     const int n_p = bf.path_len[q] - cut - pref;             // points the velocity kernel worked on
     const size_t pplane = (size_t)LTPL_NSLOT * B * dm.p_max;
     const double* E = bf.path + 4 * pplane + (size_t)q * dm.p_max + cut;
@@ -412,13 +414,12 @@ k_backup(const __grid_constant__ LtplParams prm, const __grid_constant__ LtplDim
     if (!(st & LTPL_ST_TRAJ_VALID) || !(st & LTPL_ST_VEL_BOUND_VIOL) ||
         !(act == LTPL_ACT_FOLLOW || act == LTPL_ACT_STRAIGHT))
         return;
-    if (bf.const_len[b] == 0 || bf.st_info[8 * (size_t)b] < 0) return;   // invalid last solution or restart: no backup
-                                                                         // plan (OTH:339-344)
+    if (!has_last_solution(bf, b)) return;   // no backup plan (OTH:339-344)
     const int pa = bf.prev_action_id[q];
     if (!(pa == LTPL_ACT_FOLLOW || pa == LTPL_ACT_STRAIGHT)) return;   // no backup plan: stays flagged
-    const int m_b = bf.prev_trim[4 * q + 0], L_b = bf.prev_trim[4 * q + 1];
+    const int m_b = bf.prev_trim[q].m, L_b = bf.prev_trim[q].L;
     const int n_bk = bf.prev_path_len[q] - m_b, nn_bk = bf.prev_n_nodes[q] - L_b;
-    const int cut = bf.trim[4 * q + 2], pref = bf.trim[4 * q + 3];
+    const int cut = bf.trim[q].cut, pref = bf.trim[q].pref;
     const int n_p = n_bk - cut - pref;                     // points of the brake profile
     if (n_p < 1 || nn_bk < 1) return;
     const size_t pplane = (size_t)LTPL_NSLOT * B * dm.p_max;
@@ -476,6 +477,6 @@ k_backup(const __grid_constant__ LtplParams prm, const __grid_constant__ LtplDim
             w = wn;
         }
         bf.traj_len[q] = min(n_p, dm.n_export);                 // k_prefix adds the vel_course rows
-        atomicAnd(&bf.sc_flags[b], ~(LTPL_SC_STATE_FALLBACK | (7 << LTPL_SC_REASON_SHIFT)));    // handled
+        atomicAnd(&bf.sc_flags[b], ~(LTPL_SC_STATE_FALLBACK | LTPL_SC_REASON_MASK));    // handled
     }
 }

@@ -41,7 +41,7 @@ k_export(const __grid_constant__ LtplDims dm, const __grid_constant__ LtplBuffer
     if (e < 0) return;
     const int n = bf.traj_len[q];
     const size_t pplane = (size_t)LTPL_NSLOT * B * dm.p_max;
-    const int cut = bf.trim ? bf.trim[4 * q + 2] : 0;   // stateful tick: the trajectory starts at the cut index (OTH:700)
+    const int cut = trim_cut(bf, q);   // stateful tick: the trajectory starts at the cut index (OTH:700)
     const double* pp = bf.path + (size_t)q * dm.p_max + cut;
     const double* sv = bf.s_vx_ax + (size_t)q * dm.p_max;
     float* out = bf.traj + (size_t)e * dm.n_export * 7;

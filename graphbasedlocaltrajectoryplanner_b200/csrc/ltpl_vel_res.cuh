@@ -434,8 +434,8 @@ k_vel_res(const LatDev lt, const LtplParams prm, const LtplDims dm, const LtplBu
         int n = live ? bf.path_len[q] : 0;
         int off_in = 0, pref = 0;
         if (STATE && live) {
-            pref = bf.trim[4 * q + 3];
-            off_in = bf.trim[4 * q + 2] + pref;
+            pref = bf.trim[q].pref;
+            off_in = bf.trim[q].cut + pref;
             n = max(n - off_in, 0);
         }
         if (live && bf.vel[q % B] > prm.vel_max + 0.1) {   // VPFB:106 brake prefix: the reference raises (DESIGN.md 7)
@@ -844,12 +844,10 @@ k_vel_res(const LatDev lt, const LtplParams prm, const LtplDims dm, const LtplBu
         if (follow_cls && red) vel_bound = fabs(sqrt((double)s_wf0[pl]) - vel_plan) < prm.v_max_offset;
         if (!vel_bound) st |= LTPL_ST_VEL_BOUND_VIOL;
         // stateful tick: a backup plan exists (OTH:325-344), so a straight / follow profile that breaks the bound is
-        // replaced by a brake profile on the OLD path (OTH:950-1006): flag here, k_backup plans it and clears the flag (no
-        // backup plan exists after an invalid last solution, const_len == 0, or a restart, st_info[0] < 0: the profile is
-        // kept, OTH:945-948)
-        if (STATE && !vel_bound && (action == LTPL_ACT_FOLLOW || action == LTPL_ACT_STRAIGHT) && bf.const_len[b] != 0 &&
-            bf.st_info[8 * (size_t)b] >= 0)
-            atomicOr(&bf.sc_flags[b], LTPL_SC_STATE_FALLBACK | (6 << LTPL_SC_REASON_SHIFT));
+        // replaced by a brake profile on the OLD path (OTH:950-1006): flag here, k_backup plans it and clears the flag
+        // (without a last solution no backup plan exists: the profile is kept, OTH:945-948)
+        if (STATE && !vel_bound && (action == LTPL_ACT_FOLLOW || action == LTPL_ACT_STRAIGHT) && has_last_solution(bf, b))
+            atomicOr(&bf.sc_flags[b], LTPL_SC_STATE_FALLBACK | (LTPL_SC_REASON_NO_BACKUP << LTPL_SC_REASON_SHIFT));
         if (vel_bound || action == LTPL_ACT_FOLLOW || action == LTPL_ACT_STRAIGHT) {
             st |= LTPL_ST_TRAJ_VALID;
             bf.traj_len[q] = min(n, dm.n_export);

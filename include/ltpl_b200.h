@@ -59,14 +59,19 @@ extern "C" {
 #define LTPL_SC_STATE_FALLBACK   (1 << 4)  /* stateful tick: the last executed trajectory is not usable as memory       */
                                            /* (see the reason codes; re-anchor with ltpl_set_startpos_batch, or restart     */
                                            /* the scenario alone with buffers.restart)                                      */
-#define LTPL_SC_REASON_SHIFT 8             /* bits 8..10: why STATE_FALLBACK was raised (diagnostic detail):            */
-                                           /* 1 the executed action is not in the memory and the last tick was not      */
-                                           /*   planned either (an action the last tick merely did not return is        */
-                                           /*   planned per OTH:393-407), 2 its trajectory has <= 2 rows, 3 fewer than  */
-                                           /*   2 memory nodes, 4 the start node is the placeholder, 5 the constant     */
-                                           /*   segment exceeds p_max, 6 follow / straight cannot start at the planned  */
-                                           /*   velocity and no backup plan exists, 7 the position estimate lies at the */
-                                           /*   last row of the last trajectory (np.argmin of an empty array, OTH:570)  */
+#define LTPL_SC_REASON_SHIFT 8             /* bits 8..10: why STATE_FALLBACK was raised (diagnostic detail), one of:    */
+#define LTPL_SC_REASON_MASK (7 << LTPL_SC_REASON_SHIFT)
+#define LTPL_SC_REASON_NOT_IN_MEMORY 1     /* the executed action is not in the memory and the last tick was not        */
+                                           /* planned either (an action the last tick merely did not return is          */
+                                           /* planned per OTH:393-407)                                                  */
+#define LTPL_SC_REASON_SHORT_TRAJ    2     /* its trajectory has <= 2 rows                                              */
+#define LTPL_SC_REASON_FEW_NODES     3     /* fewer than 2 memory nodes                                                 */
+#define LTPL_SC_REASON_PLACEHOLDER   4     /* the start node is the placeholder                                         */
+#define LTPL_SC_REASON_CONST_LONG    5     /* the constant segment exceeds p_max                                        */
+#define LTPL_SC_REASON_NO_BACKUP     6     /* follow / straight cannot start at the planned velocity and no backup plan */
+                                           /* exists                                                                    */
+#define LTPL_SC_REASON_LAST_ROW      7     /* the position estimate lies at the last row of the last trajectory         */
+                                           /* (np.argmin of an empty array, OTH:570)                                    */
 #define LTPL_SC_BRAKE_PREFIX     (1 << 3)  /* vel_plan > vel_max + 0.1: the reference path raises here (OTH:747-754,   */
                                            /* 830/919 column_stack length mismatch); reported instead of planned       */
 
@@ -184,6 +189,25 @@ typedef struct LtplDims {
 } LtplDims;
 #define LTPL_MAX_SUB 8
 
+/* stateful tick (DESIGN.md section 11): what k_state found in the iterative memory of one scenario, 32 bytes            */
+typedef struct LtplStateInfo {
+    int32_t prev_q;            /* path id q of the executed trajectory in the previous buffer set, or                     */
+                               /* LTPL_STATE_RESTARTED: set_startpos's constant segment, planned like a first tick        */
+    int32_t prev_m, prev_L;    /* its trim: first memory point, first memory node                                         */
+    int32_t const_nodes;       /* entries of the node / node-index / coefficient lists in front of the start node          */
+    int32_t n_factored;        /* edges of the remaining last solution with a cost factor (GLNT:155-162)                   */
+    int32_t factored_edge[3];  /* their lattice edge ids; entry i gets w_last_edges[i], -1: edge not in the lattice       */
+} LtplStateInfo;
+#define LTPL_STATE_RESTARTED (-1)
+
+/* stateful tick: where path q of this tick is cut (OTH:586-598, 705-731), 16 bytes; zero after a first tick            */
+typedef struct LtplTrim {
+    int32_t m;     /* first memory point (path-plane index)                                                              */
+    int32_t L;     /* first memory node (node index)                                                                     */
+    int32_t cut;   /* first trajectory point (path-plane index)                                                          */
+    int32_t pref;  /* points of vel_course in front of the new velocity profile                                          */
+} LtplTrim;
+
 /* Caller-owned device buffers.  q = slot * B + b indexes a path ("action major").                                      */
 typedef struct LtplBuffers {
     /* scenario inputs (Graph_LTPL.set_startpos / calc_paths arguments)                                                 */
@@ -256,16 +280,13 @@ typedef struct LtplBuffers {
     const double* prev_s_vx_ax;     /* ... `s_vx_ax` (rows 0 .. traj_len-1 = the exported trajectory = __last_bp_action_set) */
     const int32_t* prev_action_id;  /* ... `action_id`                                                                    */
     const int32_t* prev_traj_len;   /* ... `traj_len`                                                                     */
-    const int32_t* prev_trim;       /* ... `trim`                                                                         */
+    const LtplTrim* prev_trim;      /* ... `trim`                                                                         */
     const int32_t* sel_action;      /* [B] LTPL_ACT_* the caller executed since the previous tick (prev_action_id)        */
     const double* pos_last;         /* [B][2] pos_est of the previous calc_vel_profile call (OTH:537, MOPG:80-84)         */
     const double* t_const;          /* [B] min(average calculation time * calc_time_safety, 0.5) (OTH:353-375): the host  */
                                     /*     keeps the moving average, so the wall clock is an input                         */
-    int32_t* st_info;               /* [B][8] k_state: prev path id, prev m, prev L, constant nodes, #factored edges, e0..e2 */
-                                    /*     (prev path id -1: restarted, planned like a first tick)                         */
-    int32_t* trim;                  /* [NSLOT*B][4] m = first memory point, L = first memory node, c = first trajectory   */
-                                    /*     point (path-plane indices of THIS tick, OTH:586-598, 705-731), pref = #points    */
-                                    /*     of vel_course; set to zero by a first tick                                       */
+    LtplStateInfo* st_info;         /* [B] written by k_state                                                             */
+    LtplTrim* trim;                 /* [NSLOT*B]                                                                          */
     double* vel_plan;               /* [B] planned velocity at the cut (OTH:572): the start of the velocity profiles      */
     double* course;                 /* [B][n_export] vel_course (OTH:574): at most the rows of an exported trajectory      */
     double* obj_dist;               /* [B] s_obj - s_start on the cut follow path (OTH:774-784)                            */

@@ -24,6 +24,11 @@ def test_capi_library_exports_every_declared_symbol():
     assert lib.ltpl_version() == capi.ABI_VERSION
     for which, st in enumerate((capi.LatticeHeader, capi.Params, capi.Dims, capi.Buffers, capi.VelBatch)):
         assert lib.ltpl_sizeof(which) == ctypes.sizeof(st)
+    # scenario flags and fallback reason codes: the header's values (in order, each may use the ones before) == capi's
+    sc = {}
+    for name, expr in re.findall(r"^#define LTPL_(SC_\w+)\s+([^/\n]+)", header, flags=re.M):
+        sc[name] = eval(re.sub(r"\bLTPL_(SC_\w+)", r"\1", expr), {"__builtins__": {}}, dict(sc))
+    assert sc == {n: getattr(capi, n) for n in dir(capi) if n.startswith("SC_")}, sc
     # error convention without touching a GPU: null arguments are rejected with a message
     assert lib.ltpl_lattice_create(None, None, None) != 0
     assert b"null" in lib.ltpl_last_error()

@@ -83,7 +83,7 @@ def main():
         flags = f["sc_flags"]
         new = (flags != 0) & ~seen
         seen |= flags != 0
-        reason = (flags >> 8) & 7
+        reason = (flags & capi.SC_REASON_MASK) >> capi.SC_REASON_SHIFT
         hist = collections.Counter()
         for b in np.nonzero(new)[0]:
             hist[("capacity" if flags[b] & capi.SC_CAPACITY else "reason%d" % reason[b])] += 1
