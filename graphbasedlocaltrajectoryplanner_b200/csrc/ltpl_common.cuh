@@ -108,6 +108,60 @@ __device__ __forceinline__ int sub_path(const LtplDims& dm, int warps_per_cta) {
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
+// rows of the per-path and per-scenario buffers of LtplBuffers: these views implement the layout comments of
+// include/ltpl_b200.h
+// ---------------------------------------------------------------------------------------------------------------------
+enum PathCol { PATH_X, PATH_Y, PATH_PSI, PATH_KAPPA, PATH_EL };   // planes of path, prev_path and const_seg
+enum SvaCol { SVA_S, SVA_VX, SVA_AX };                             // planes of s_vx_ax and prev_s_vx_ax
+enum GgCol { GG_AX, GG_AY };                                       // planes of gg and prev_gg
+enum TrajCol { TRAJ_S, TRAJ_X, TRAJ_Y, TRAJ_PSI, TRAJ_KAPPA, TRAJ_VX, TRAJ_AX, TRAJ_COLS };   // columns of a traj point
+
+// one row of a plane-major buffer from some point on: point i of plane c
+template <class T>
+struct PlaneRow {
+    T* p;           // plane 0
+    size_t plane;   // elements from one plane to the next
+    __device__ __forceinline__ T* col(int c) const { return p + c * plane; }
+    __device__ __forceinline__ T& operator()(int c, int i) const { return p[c * plane + i]; }
+};
+// path q of path, s_vx_ax, gg or their prev_ ([NSLOT*B][p_max] per plane), from point i0 on
+template <class T>
+__device__ __forceinline__ PlaneRow<T> path_row(T* base, const LtplDims& dm, int q, int i0 = 0) {
+    return {base + (size_t)q * dm.p_max + i0, (size_t)LTPL_NSLOT * dm.batch * dm.p_max};
+}
+// scenario b of const_seg ([5][B][p0_max])
+template <class T>
+__device__ __forceinline__ PlaneRow<T> const_seg_row(T* base, const LtplDims& dm, int b) {
+    return {base + (size_t)b * dm.p0_max, (size_t)dm.batch * dm.p0_max};
+}
+
+// the h_max-entry lists of path q from entry j on: node_idx and edge_seq (one int), nodes ((layer, node) pairs), coeff
+// (x(4) | y(4)); also for the prev_ lists
+template <class T>
+__device__ __forceinline__ T* list_row(T* base, const LtplDims& dm, int q, int j = 0) {
+    return base + (size_t)q * dm.h_max + j;
+}
+template <class T>
+__device__ __forceinline__ T* node_row(T* base, const LtplDims& dm, int q, int j = 0) {
+    return base + ((size_t)q * dm.h_max + j) * 2;
+}
+template <class T>
+__device__ __forceinline__ T* coeff_row(T* base, const LtplDims& dm, int q, int j = 0) {
+    return base + ((size_t)q * dm.h_max + j) * 8;
+}
+
+// the n_export rows of scenario b in course, em_vx and prev_em_vx
+template <class T>
+__device__ __forceinline__ T* scenario_row(T* base, const LtplDims& dm, int b) {
+    return base + (size_t)b * dm.n_export;
+}
+
+// row e of traj: n_export points of TRAJ_COLS floats
+__device__ __forceinline__ float* traj_row(const LtplDims& dm, const LtplBuffers& bf, int e) {
+    return bf.traj + (size_t)e * dm.n_export * TRAJ_COLS;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
 // the iterative memory of a stateful tick as k_state left it (LtplStateInfo, LtplTrim)
 // ---------------------------------------------------------------------------------------------------------------------
 // a valid last solution: neither an executed action the last tick did not return (const_len == 0, OTH:393-407) nor a
@@ -138,7 +192,7 @@ struct ConstView {
 template <bool STATE>
 __device__ __forceinline__ ConstView const_view(const LtplDims& dm, const LtplBuffers& bf, int b, int B) {
     ConstView v;
-    v.plane = (size_t)B * dm.p0_max;
+    v.plane = (size_t)B * dm.p0_max;   // const_seg_row, but with the caller's B: re-read from dm, k_plan spills
     v.seg = bf.const_seg + (size_t)b * dm.p0_max;
     v.m = v.rows = 0;
     v.nodes = v.node_idx = nullptr;
@@ -146,14 +200,14 @@ __device__ __forceinline__ ConstView const_view(const LtplDims& dm, const LtplBu
     v.mem = STATE && bf.st_info[b].prev_q >= 0;
     if (v.mem) {
         const LtplStateInfo& si = bf.st_info[b];
-        const size_t row = (size_t)si.prev_q * dm.h_max + si.prev_L;
-        v.plane = (size_t)LTPL_NSLOT * B * dm.p_max;
-        v.seg = bf.prev_path + (size_t)si.prev_q * dm.p_max + si.prev_m;
+        const PlaneRow<const double> mp = path_row(bf.prev_path, dm, si.prev_q, si.prev_m);
+        v.seg = mp.p;
+        v.plane = mp.plane;
         v.m = si.prev_m;
         v.rows = bf.prev_n_nodes[si.prev_q] - si.prev_L - 1;
-        v.nodes = bf.prev_nodes + row * 2;
-        v.node_idx = bf.prev_node_idx + row;
-        v.coeff = bf.prev_coeff + row * 8;
+        v.nodes = node_row(bf.prev_nodes, dm, si.prev_q, si.prev_L);
+        v.node_idx = list_row(bf.prev_node_idx, dm, si.prev_q, si.prev_L);
+        v.coeff = coeff_row(bf.prev_coeff, dm, si.prev_q, si.prev_L);
     }
     return v;
 }

@@ -102,8 +102,7 @@ k_startpos(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams
         return;
     }
     const double dstep = len / (double)(p0 - 1);
-    const size_t plane = (size_t)dm.batch * dm.p0_max;
-    double* cs = bf.const_seg + (size_t)b * dm.p0_max;
+    const PlaneRow<double> cs = const_seg_row(bf.const_seg, dm, b);
     #pragma unroll 1
     for (int k = lane; k < p0; k += 32) {
         double t, x, y, tn, xn, yn;
@@ -130,11 +129,11 @@ k_startpos(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams
         }
         double psi, kap;
         head_curv(ax1, ax2, ax3, ay1, ay2, ay3, t, &psi, &kap);
-        cs[0 * plane + k] = x;
-        cs[1 * plane + k] = y;
-        cs[2 * plane + k] = psi;
-        cs[3 * plane + k] = kap;
-        cs[4 * plane + k] = elk;
+        cs(PATH_X, k) = x;
+        cs(PATH_Y, k) = y;
+        cs(PATH_PSI, k) = psi;
+        cs(PATH_KAPPA, k) = kap;
+        cs(PATH_EL, k) = elk;
     }
     if (lane == 0) {
         bf.sc_flags[b] = flags;

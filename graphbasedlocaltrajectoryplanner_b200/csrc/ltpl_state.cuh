@@ -128,11 +128,12 @@ k_state(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams pr
     }
     const LtplTrim& tp = bf.prev_trim[qp];
     const int m_p = tp.m, L_p = tp.L, c_p = tp.cut;
-    const size_t pplane = (size_t)LTPL_NSLOT * B * dm.p_max;
-    const double* Px = bf.prev_path + (size_t)qp * dm.p_max;
-    const double* Py = Px + pplane;
-    const double* S = bf.prev_s_vx_ax + (size_t)qp * dm.p_max;
-    const double* V = S + pplane;
+    const PlaneRow<const double> path = path_row(bf.prev_path, dm, qp);
+    const double* Px = path.col(PATH_X);
+    const double* Py = path.col(PATH_Y);
+    const PlaneRow<const double> sv = path_row(bf.prev_s_vx_ax, dm, qp);
+    const double* S = sv.col(SVA_S);
+    const double* V = sv.col(SVA_VX);
 
     // index of the pose on the last trajectory after t_const (OTH:366-378; quirk q11: ds / v with inf where v == 0)
     int next_idx = 1;
@@ -160,8 +161,8 @@ k_state(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams pr
         if (lane == 0) bf.sc_flags[b] = LTPL_SC_STATE_FALLBACK | (LTPL_SC_REASON_FEW_NODES << LTPL_SC_REASON_SHIFT);
         return;
     }
-    const int* Ip = bf.prev_node_idx + (size_t)qp * dm.h_max + L_p;
-    const int* Np = bf.prev_nodes + ((size_t)qp * dm.h_max + L_p) * 2;
+    const int* Ip = list_row(bf.prev_node_idx, dm, qp, L_p);
+    const int* Np = node_row(bf.prev_nodes, dm, qp, L_p);
     const int2 pair = open_index_pair([&](int i) { const int pi = Ip[i]; return make_double2(Px[pi], Py[pi]); },
                                       nn_mem, ppx, ppy, lane);
     const int sni = pair.y;                          // start_node_idx within the memory node list
@@ -199,16 +200,15 @@ k_state(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams pr
 // follow mode: distance to the closest object along the cut follow path (OTH:766-784); no object -> 0 (OTH:766-768)
 __device__ __forceinline__ void ref_obj_dist(const LtplDims& dm, const LtplBuffers& bf, int b, int cut_pos, double px,
                                              double py, int lane) {
-    const int B = dm.batch;
-    const size_t pplane = (size_t)LTPL_NSLOT * B * dm.p_max;
+    const int qf = b;   // slot 0
+    const PlaneRow<const double> path = path_row<const double>(bf.path, dm, qf, cut_pos);
     if (lane == 0) bf.obj_dist[b] = 0.0;
     __syncwarp();
-    const int qf = b;   // slot 0
     if (bf.action_id[qf] == LTPL_ACT_FOLLOW && bf.closest_obj[b] >= 0) {
         const int n = bf.path_len[qf] - cut_pos;
-        const double* X = bf.path + (size_t)qf * dm.p_max + cut_pos;
-        const double* Y = X + pplane;
-        const double* E = X + 4 * pplane;
+        const double* X = path.col(PATH_X);
+        const double* Y = path.col(PATH_Y);
+        const double* E = path.col(PATH_EL);
         double s_two[2];
 #pragma unroll 1
         for (int w = 0; w < 2; ++w) {
@@ -265,31 +265,19 @@ k_ref(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm,
     const int qp = bf.st_info[b].prev_q, m_p = bf.st_info[b].prev_m;
     const int c_p = bf.prev_trim[qp].cut;
     const int nb_rows = bf.prev_traj_len[qp];
-    const size_t pplane = (size_t)LTPL_NSLOT * B * dm.p_max;
-    const double* Px = bf.prev_path + (size_t)qp * dm.p_max + c_p;   // trajectory row j -> path point c + j
-    const double* Py = Px + pplane;
-    const double* S = bf.prev_s_vx_ax + (size_t)qp * dm.p_max;
-    const double* V = S + pplane;
+    const PlaneRow<const double> path = path_row(bf.prev_path, dm, qp, c_p);   // trajectory row j -> path point c + j
+    const double* Px = path.col(PATH_X);
+    const double* Py = path.col(PATH_Y);
+    const PlaneRow<const double> sv = path_row(bf.prev_s_vx_ax, dm, qp);
+    const double* S = sv.col(SVA_S);
+    const double* V = sv.col(SVA_VX);
     // an executed 'emergency' trajectory shares s, x, y with its base (calc_brake_emergency.py:40-45) but not the velocity
-    if (bf.sel_action[b] == LTPL_ACT_EMERGENCY) V = bf.prev_em_vx + (size_t)b * dm.n_export;
+    if (bf.sel_action[b] == LTPL_ACT_EMERGENCY) V = scenario_row(bf.prev_em_vx, dm, b);
     const double px = bf.pos[2 * b], py = bf.pos[2 * b + 1];
 
     // cut index: first of the two trajectory points around pos_est (OTH:551-556); n_export <= 128 rows
-    double bv = LTPL_INF;
-    int bi = 0x7fffffff;
-    for (int j = lane; j < nb_rows; j += 32) {
-        const double d = dist2_rn(Px[j], Py[j], px, py);
-        if (d < bv) {
-            bv = d;
-            bi = j;
-        }
-    }
-    const ArgMinD mm = warp_argmin(bv, bi);
-    const int nb = mm.i;
-    const int idx1 = max(nb - 1, 0), idx2 = min(nb + 1, nb_rows - 1);
-    const AngCmp ac = angle_cmp(make_double2(Px[nb], Py[nb]), px, py, make_double2(Px[idx1], Py[idx1]),
-                                make_double2(Px[idx2], Py[idx2]));
-    const int cut_index = ac.ge ? idx1 : nb;
+    const int cut_index =
+        open_index_pair([&](int j) { return make_double2(Px[j], Py[j]); }, nb_rows, px, py, lane).x;
 
     // delay compensation (OTH:558-574)
     int vel_idx = 1;
@@ -310,7 +298,7 @@ k_ref(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm,
         if (vel_idx >= 0) {
             bf.vel_plan[b] = V[cut_index + vel_idx];
             // `course` holds n_export rows per scenario = as many as an exported trajectory has: no truncation
-            for (int i = 0; i < vel_idx; ++i) bf.course[(size_t)b * dm.n_export + i] = V[cut_index + i];
+            for (int i = 0; i < vel_idx; ++i) scenario_row(bf.course, dm, b)[i] = V[cut_index + i];
         }
     }
     vel_idx = __shfl_sync(LTPL_FULL, vel_idx, 0);
@@ -327,7 +315,7 @@ k_ref(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm,
     int cut_layer = 0;
     if (q0 >= 0) {
         const int nn = bf.n_nodes[q0];
-        const int* ni = bf.node_idx + (size_t)q0 * dm.h_max;
+        const int* ni = list_row(bf.node_idx, dm, q0);
         int first = nn;                              // np.argmin(node_idx < cut_pos): first index with node_idx >= cut_pos
         for (int i = lane; i < nn; i += 32)
             if (!(ni[i] < cut_pos)) first = min(first, i);
@@ -340,7 +328,7 @@ k_ref(const __grid_constant__ LatDev lt, const __grid_constant__ LtplParams prm,
         const int q = lane * B + b;
         LtplTrim& tr = bf.trim[q];
         if (bf.action_id[q] != LTPL_ACT_NONE) {
-            tr.m = bf.node_idx[(size_t)q * dm.h_max + cut_layer];
+            tr.m = list_row(bf.node_idx, dm, q)[cut_layer];
             tr.L = cut_layer;
             tr.cut = cut_pos;
             tr.pref = vel_idx;
@@ -368,11 +356,12 @@ k_prefix(const __grid_constant__ LtplDims dm, const __grid_constant__ LtplBuffer
     const int b = q % B;
     const int cut = bf.trim[q].cut, pref = bf.trim[q].pref;
     const int n_p = bf.path_len[q] - cut - pref;             // points the velocity kernel worked on
-    const size_t pplane = (size_t)LTPL_NSLOT * B * dm.p_max;
-    const double* E = bf.path + 4 * pplane + (size_t)q * dm.p_max + cut;
-    double* S = bf.s_vx_ax + (size_t)q * dm.p_max;
-    double* VX = S + pplane;
-    double* AX = VX + pplane;
+    const double* E = path_row<const double>(bf.path, dm, q, cut).col(PATH_EL);
+    const PlaneRow<double> sv = path_row(bf.s_vx_ax, dm, q);
+    double* S = sv.col(SVA_S);
+    double* VX = sv.col(SVA_VX);
+    double* AX = sv.col(SVA_AX);
+    const double* course = scenario_row(bf.course, dm, b);
     double s_pref = 0.0;
     for (int j = 0; j < pref; ++j) s_pref = __dadd_rn(s_pref, E[j]);
     for (int i = pref + lane; i < pref + n_p; i += 32) S[i] += s_pref;
@@ -381,7 +370,7 @@ k_prefix(const __grid_constant__ LtplDims dm, const __grid_constant__ LtplBuffer
         double acc = 0.0;
         for (int i = 0; i < pref; ++i) {
             S[i] = acc;
-            VX[i] = bf.course[(size_t)b * dm.n_export + i];
+            VX[i] = course[i];
             acc = __dadd_rn(acc, E[i]);
         }
         for (int i = 0; i < pref; ++i) {
@@ -407,7 +396,6 @@ k_backup(const __grid_constant__ LtplParams prm, const __grid_constant__ LtplDim
     const int lane = threadIdx.x & 31;
     const int b = sub_scenario(dm, LTPL_WARPS_PER_CTA);
     if (b < 0) return;
-    const int B = dm.batch;
     const int q = b;   // slot 0: follow / straight
     const int st = bf.status[q];
     const int act = bf.action_id[q];
@@ -422,33 +410,37 @@ k_backup(const __grid_constant__ LtplParams prm, const __grid_constant__ LtplDim
     const int cut = bf.trim[q].cut, pref = bf.trim[q].pref;
     const int n_p = n_bk - cut - pref;                     // points of the brake profile
     if (n_p < 1 || nn_bk < 1) return;
-    const size_t pplane = (size_t)LTPL_NSLOT * B * dm.p_max;
     // the backup becomes this tick's memory (OTH:958-963); the trims of k_ref stay (they are what the slices use)
-    for (int c = 0; c < 5; ++c) {
-        const double* src = bf.prev_path + c * pplane + (size_t)q * dm.p_max + m_b;
-        double* dst = bf.path + c * pplane + (size_t)q * dm.p_max;
-        for (int i = lane; i < n_bk; i += 32) dst[i] = src[i];
-    }
+    const PlaneRow<const double> src = path_row(bf.prev_path, dm, q, m_b);
+    const PlaneRow<double> dst = path_row(bf.path, dm, q);
+    for (int c = PATH_X; c <= PATH_EL; ++c)
+        for (int i = lane; i < n_bk; i += 32) dst(c, i) = src(c, i);
+    const int* src_idx = list_row(bf.prev_node_idx, dm, q, L_b);
+    const int* src_nodes = node_row(bf.prev_nodes, dm, q, L_b);
+    int* dst_nodes = node_row(bf.nodes, dm, q);
     for (int j = lane; j < nn_bk; j += 32) {
-        bf.node_idx[(size_t)q * dm.h_max + j] = bf.prev_node_idx[(size_t)q * dm.h_max + L_b + j] - m_b;
-        bf.nodes[((size_t)q * dm.h_max + j) * 2] = bf.prev_nodes[((size_t)q * dm.h_max + L_b + j) * 2];
-        bf.nodes[((size_t)q * dm.h_max + j) * 2 + 1] = bf.prev_nodes[((size_t)q * dm.h_max + L_b + j) * 2 + 1];
+        list_row(bf.node_idx, dm, q)[j] = src_idx[j] - m_b;
+        dst_nodes[2 * j] = src_nodes[2 * j];
+        dst_nodes[2 * j + 1] = src_nodes[2 * j + 1];
     }
     for (int j = lane; j < max(nn_bk - 1, 1) * 8; j += 32)
-        bf.coeff[(size_t)q * dm.h_max * 8 + j] = bf.prev_coeff[((size_t)q * dm.h_max + L_b) * 8 + j];
+        coeff_row(bf.coeff, dm, q)[j] = coeff_row(bf.prev_coeff, dm, q, L_b)[j];
     __syncwarp();
     if (lane == 0) {
         bf.path_len[q] = n_bk;
         bf.n_nodes[q] = nn_bk;
         // full braking from the planned velocity behind vel_course (tph.calc_vel_profile_brake, mode 'decel_forw')
-        const double* K = bf.path + 3 * pplane + (size_t)q * dm.p_max + cut + pref;
-        const double* E = K + pplane;
-        double* S = bf.s_vx_ax + (size_t)q * dm.p_max + pref;   // rows behind vel_course, arc length 0 at their first point
-        double* VX = S + pplane;
-        double* AX = VX + pplane;
+        const PlaneRow<const double> path = path_row<const double>(bf.path, dm, q, cut + pref);
+        const double* K = path.col(PATH_KAPPA);
+        const double* E = path.col(PATH_EL);
+        const PlaneRow<double> sv = path_row(bf.s_vx_ax, dm, q, pref);   // rows behind vel_course, arc length 0 at their first point
+        double* S = sv.col(SVA_S);
+        double* VX = sv.col(SVA_VX);
+        double* AX = sv.col(SVA_AX);
         const double dmq = prm.drag_coeff / prm.m_veh, inv_ay = 1.0 / prm.gg_ay;
         // location dependent local_gg of the LAST tick along the backup path (__backup_path_gg, OTH:970-975), raw
-        const double* ggr = bf.prev_gg ? bf.prev_gg + (size_t)q * dm.p_max + m_b + cut + pref : nullptr;
+        const PlaneRow<const double> ggr =
+            bf.prev_gg ? path_row(bf.prev_gg, dm, q, m_b + cut + pref) : PlaneRow<const double>{nullptr, 0};
         double v0 = bf.vel[b];                                  // == vel_plan (run_tick launches k_backup so)
         if (v0 < 0.0) v0 = 0.0;
         double w = v0 * v0, s = 0.0;
@@ -459,8 +451,9 @@ k_backup(const __grid_constant__ LtplParams prm, const __grid_constant__ LtplDim
             double wn = 0.0;
             if (i + 1 < n_p) {
                 if (!stopped) {
-                    const double a = ggr ? acc_brake(w, fabs(K[i]), ggr[i], 1.0 / ggr[pplane + i], prm.dyn_model_exp, dmq)
-                                         : acc_brake(w, fabs(K[i]), prm.gg_ax, inv_ay, prm.dyn_model_exp, dmq);
+                    const double a =
+                        ggr.p ? acc_brake(w, fabs(K[i]), ggr(GG_AX, i), 1.0 / ggr(GG_AY, i), prm.dyn_model_exp, dmq)
+                              : acc_brake(w, fabs(K[i]), prm.gg_ax, inv_ay, prm.dyn_model_exp, dmq);
                     const double nx = fma(2.0 * a, E[i], w);
                     if (nx < 0.0)
                         stopped = true;

@@ -33,27 +33,25 @@ __device__ __forceinline__ double acc_brake(double w, double kabs, double ax_max
 // (P, 7) rows s, x, y, psi, kappa, vx, ax of every kept trajectory, cut to nmbr_export_points (OTH:941, LTPL:401-406)
 __global__ void __launch_bounds__(LTPL_WARPS_PER_CTA_EXPORT * 32)
 k_export(const __grid_constant__ LtplDims dm, const __grid_constant__ LtplBuffers bf) {
-    const int B = dm.batch;
     const int lane = threadIdx.x & 31;
     const int q = sub_path(dm, LTPL_WARPS_PER_CTA_EXPORT);   // a path of this launch's window ...
     if (q < 0) return;
     const int e = bf.traj_row[q];                            // ... and its row of the compact export list
     if (e < 0) return;
     const int n = bf.traj_len[q];
-    const size_t pplane = (size_t)LTPL_NSLOT * B * dm.p_max;
     const int cut = trim_cut(bf, q);   // stateful tick: the trajectory starts at the cut index (OTH:700)
-    const double* pp = bf.path + (size_t)q * dm.p_max + cut;
-    const double* sv = bf.s_vx_ax + (size_t)q * dm.p_max;
-    float* out = bf.traj + (size_t)e * dm.n_export * 7;
-    for (int i = lane; i < n * 7; i += 32) {
-        const int r = i / 7, col = i - 7 * r;
+    const PlaneRow<const double> pp = path_row<const double>(bf.path, dm, q, cut);
+    const PlaneRow<const double> sv = path_row<const double>(bf.s_vx_ax, dm, q);
+    float* out = traj_row(dm, bf, e);
+    for (int i = lane; i < n * TRAJ_COLS; i += 32) {   // the points of a row are contiguous
+        const int r = i / TRAJ_COLS, col = i - TRAJ_COLS * r;
         double v;
-        if (col == 0)
-            v = sv[r];
-        else if (col <= 4)
-            v = pp[(size_t)(col - 1) * pplane + r];
+        if (col == TRAJ_S)
+            v = sv(SVA_S, r);
+        else if (col <= TRAJ_KAPPA)
+            v = pp(col - TRAJ_X + PATH_X, r);
         else
-            v = sv[(size_t)(col - 4) * pplane + r];
+            v = sv(col - TRAJ_VX + SVA_VX, r);
         out[i] = (float)v;
     }
 }
