@@ -15,7 +15,7 @@ import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
 
 import bench  # noqa: E402
-from tests import helpers as H  # noqa: E402
+from tools.workload import step_along  # noqa: E402
 
 
 class _Clk(object):
@@ -24,15 +24,6 @@ class _Clk(object):
 
     def __call__(self):
         return self.t
-
-
-def _advance(tr, dt):
-    n = max(tr.shape[0], 2)
-    s_t = tr[0, 0] + max(tr[0, 5] * dt + 0.5 * tr[0, 6] * dt * dt, 0.0)
-    i0 = int(np.clip((tr[:, 0] <= s_t).sum() - 1, 0, n - 2))
-    f = float(np.clip((s_t - tr[i0, 0]) / max(tr[i0 + 1, 0] - tr[i0, 0], 1e-9), 0.0, 1.0))
-    lerp = lambda c: tr[i0, c] * (1 - f) + tr[i0 + 1, c] * f   # noqa: E731
-    return np.array([lerp(1), lerp(2)]), lerp(5)
 
 
 def _run(args):
@@ -78,7 +69,8 @@ def _run(args):
                 t = traj[sel][0]
                 if t.shape[0] <= 2:
                     ev.append("tick%d:short_traj(%d)" % (k, t.shape[0]))
-                pos_e, vel_e = _advance(t, 0.1)
+                p, v, _ = step_along(t[None], [t.shape[0]], 0.1)
+                pos_e, vel_e = p[0], v[0]
             except Exception as e:   # noqa: BLE001
                 ev.append("tick%d:exception(%s: %s)" % (k, type(e).__name__, str(e)[:80]))
                 break

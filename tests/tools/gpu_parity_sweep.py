@@ -1,6 +1,6 @@
 """large parity sweep (GPU box): CUDA path vs the oracle over thousands of seeded scenarios per lattice, compared with the
 rules of tests/helpers.compare_records (node sequences bit-exact, coordinates / velocities 1e-4).  The oracle runs in a
-process pool on the host cores.   python tools/gpu_parity_sweep.py [n_per_lattice] [lattice ...]"""
+process pool on the host cores.   python tests/tools/gpu_parity_sweep.py [n_per_lattice] [lattice ...] [--features]"""
 import os, sys, time
 REPO = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, REPO)

@@ -18,6 +18,7 @@ import bench  # noqa: E402
 from graphbasedlocaltrajectoryplanner_b200 import capi  # noqa: E402
 from graphbasedlocaltrajectoryplanner_b200.planner import BatchPlanner, read_online_config  # noqa: E402
 from graphbasedlocaltrajectoryplanner_b200.scenarios import ScenarioBatch  # noqa: E402
+from tools.workload import closed_loop_step  # noqa: E402
 
 
 class _Clk(object):
@@ -26,25 +27,6 @@ class _Clk(object):
 
     def __call__(self):
         return self.t
-
-
-def advance(out, dt_loop):
-    rows = out["traj_row"].numpy()
-    lens = out["traj_len"].numpy()
-    acts = out["action_id"].numpy()
-    slot = np.argmax(rows >= 0, axis=0)
-    bidx = np.arange(rows.shape[1])
-    ok = rows[slot, bidx] >= 0
-    r = np.where(ok, rows[slot, bidx], 0)
-    tr = out["traj"].numpy()[r].astype(np.float64)
-    n = np.maximum(lens[slot, bidx], 2)
-    s_t = tr[:, 0, 0] + np.maximum(tr[:, 0, 5] * dt_loop + 0.5 * tr[:, 0, 6] * dt_loop ** 2, 0.0)
-    valid = np.arange(tr.shape[1])[None, :] < n[:, None]
-    i0 = np.clip((np.where(valid, tr[:, :, 0], np.inf) <= s_t[:, None]).sum(axis=1) - 1, 0, n - 2)
-    s0, s1 = tr[bidx, i0, 0], tr[bidx, i0 + 1, 0]
-    f = np.clip((s_t - s0) / np.maximum(s1 - s0, 1e-9), 0.0, 1.0)
-    lerp = lambda c: tr[bidx, i0, c] * (1 - f) + tr[bidx, i0 + 1, c] * f   # noqa: E731
-    return np.column_stack((lerp(1), lerp(2))), lerp(5), np.where(ok, acts[slot, bidx], 0), ok
 
 
 def main():
@@ -71,12 +53,10 @@ def main():
     names = {v: k for k, v in capi.ACTION_NAMES.items()}
     inv = capi.ACTION_NAMES
     for k in range(1, a.ticks + 1):
-        out = pl.download()
-        torch.cuda.synchronize(device)
-        prev = {n: out[n].numpy().copy() for n in ("action_id", "traj_len", "status")}
-        p_new, v_new, sel_a, ok = advance(out, dt)
+        prev = pl.fetch("traj_row", "traj_len", "action_id", "traj", "status")
+        p_new, v_new, sel_a, ok, _ = closed_loop_step(prev, dt)
         pos_e, vel_e = np.where(ok[:, None], p_new, pos_e), np.where(ok, v_new, vel_e)
-        rec_in.append((pos_e.copy(), vel_e.copy(), sel_a.astype(np.int32)))
+        rec_in.append((pos_e.copy(), vel_e.copy(), sel_a))
         pl.next_tick(ScenarioBatch(pos_e.copy(), sc.heading, sc.vel, sc.n_obj, sc.obj), sel_a, 2.0 * dt, vel_est=vel_e)
         torch.cuda.synchronize(device)
         f = pl.fetch("sc_flags", "action_id", "traj_len", "status")

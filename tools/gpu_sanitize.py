@@ -2,9 +2,9 @@
 Run as  compute-sanitizer --tool memcheck|racecheck|initcheck|synccheck python tools/gpu_sanitize.py"""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import numpy as np
 from tests import helpers as H
+from tools.workload import with_objects, with_predictions
 from graphbasedlocaltrajectoryplanner_b200.planner import BatchPlanner
 from graphbasedlocaltrajectoryplanner_b200.scenarios import Track, make_scenarios, make_velocity_microbench
 from graphbasedlocaltrajectoryplanner_b200.velprofile import calc_vel_profile_batch
@@ -19,39 +19,24 @@ for tag in ("default", "l216"):
     pl.stage_scenarios(sc); pl.upload(); pl.set_startpos(); pl.tick()
     r = pl.records()
     print(tag, "trajectories:", sum(len(x.get("traj", {})) for x in r))
-# velocity smoothing (k_smooth): a first tick and a stateful tick at window 5, emergency trajectory on
+# a first tick and a stateful tick of each case: velocity smoothing (k_smooth) at window 5 with the emergency trajectory
+# on; long prediction arrays (k_plan's disc stage in chunks of 32): 3 objects x 40 points = 123 discs per scenario; long
+# object lists (k_plan's object stage in chunks of 32, a vehicle record per on-track object): 70 objects per scenario,
+# every second added one beyond the track bounds
 g = H.golden("ticks_default.npz")
-sc = make_scenarios(Track(H.TRACK_CSV), n, seed=78, n_obj_min=0, n_obj_max=3)
-ps = BatchPlanner(H.lattice_for("default"), online=dict(filt_window_width=5), device="cuda:0", stateful=True)
-ps.set_vel_params(ax_max_machines=g["ax_max_machines"], incl_emerg_traj=True, **VEL)
-ps.stage_scenarios(sc); ps.upload(); ps.set_startpos(); ps.tick()
-sel = ps.t["action_id"].max(dim=0).values.clamp(min=0).cpu().numpy()   # an action every scenario's tick returned
-ps.next_tick(sc, sel_action=sel, t_const=0.1)
-r = ps.records()
-print("smoothed stateful tick, trajectories:", sum(len(x.get("traj", {})) for x in r))
-# long prediction arrays (k_plan's disc stage in chunks of 32): 3 objects x 40 points = 123 discs per scenario, a first
-# tick and a stateful tick
-from bench_pred import with_predictions  # noqa: E402
-sc = with_predictions(make_scenarios(Track(H.TRACK_CSV), n, seed=79, n_obj_min=3, n_obj_max=3), 40)
-pp = BatchPlanner(H.lattice_for("default"), device="cuda:0", stateful=True)
-pp.set_vel_params(ax_max_machines=g["ax_max_machines"], **VEL)
-pp.stage_scenarios(sc); pp.upload(); pp.set_startpos(); pp.tick()
-sel = pp.t["action_id"].max(dim=0).values.clamp(min=0).cpu().numpy()
-pp.next_tick(sc, sel_action=sel, t_const=0.1)
-r = pp.records()
-print("long-prediction stateful tick, trajectories:", sum(len(x.get("traj", {})) for x in r))
-# long object lists (k_plan's object stage in chunks of 32, a vehicle record per on-track object): 70 objects per
-# scenario, every second added one beyond the track bounds, a first tick and a stateful tick
-from bench_objects import with_objects  # noqa: E402
 tr = Track(H.TRACK_CSV)
-sc = with_objects(make_scenarios(tr, n, seed=80, n_obj_min=1, n_obj_max=3), 70, tr)
-po = BatchPlanner(H.lattice_for("default"), device="cuda:0", stateful=True)
-po.set_vel_params(ax_max_machines=g["ax_max_machines"], **VEL)
-po.stage_scenarios(sc); po.upload(); po.set_startpos(); po.tick()
-sel = po.t["action_id"].max(dim=0).values.clamp(min=0).cpu().numpy()
-po.next_tick(sc, sel_action=sel, t_const=0.1)
-r = po.records()
-print("70-object stateful tick, trajectories:", sum(len(x.get("traj", {})) for x in r))
+for name, seed, n_obj, variant, online, emerg in (
+        ("smoothed", 78, (0, 3), lambda sc: sc, dict(filt_window_width=5), True),
+        ("long-prediction", 79, (3, 3), lambda sc: with_predictions(sc, 40), None, False),
+        ("70-object", 80, (1, 3), lambda sc: with_objects(sc, 70, tr), None, False)):
+    sc = variant(make_scenarios(tr, n, seed=seed, n_obj_min=n_obj[0], n_obj_max=n_obj[1]))
+    ps = BatchPlanner(H.lattice_for("default"), online=online, device="cuda:0", stateful=True)
+    ps.set_vel_params(ax_max_machines=g["ax_max_machines"], incl_emerg_traj=emerg, **VEL)
+    ps.stage_scenarios(sc); ps.upload(); ps.set_startpos(); ps.tick()
+    sel = ps.t["action_id"].max(dim=0).values.clamp(min=0).cpu().numpy()   # an action every scenario's tick returned
+    ps.next_tick(sc, sel_action=sel, t_const=0.1)
+    r = ps.records()
+    print(name + " stateful tick, trajectories:", sum(len(x.get("traj", {})) for x in r))
 # restarts inside a stateful tick (masked k_startpos in front of k_state): every third scenario, a few of them to a
 # pose off the track, emergency trajectory on, then a stateful tick without restarts
 sc = make_scenarios(Track(H.TRACK_CSV), n, seed=81, n_obj_min=0, n_obj_max=3)

@@ -3,20 +3,9 @@ usage: python tools/gpu_subbatch.py [tag ...]"""
 import os, sys
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, REPO)
-import torch, bench
+import bench
 from graphbasedlocaltrajectoryplanner_b200.planner import BatchPlanner
-flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
-st = torch.cuda.current_stream()
-
-
-def timed(fn, steps=12):
-    ts = []
-    for _ in range(steps):
-        flush.fill_(1)
-        e0 = torch.cuda.Event(enable_timing=True); e1 = torch.cuda.Event(enable_timing=True)
-        e0.record(st); fn(); e1.record(st); torch.cuda.synchronize(); ts.append(e0.elapsed_time(e1))
-    ts.sort()
-    return ts[len(ts) // 2]
+from tools.workload import timed_ms
 
 
 for tag in (sys.argv[1:] or ["l216", "default", "l430"]):
@@ -29,5 +18,5 @@ for tag in (sys.argv[1:] or ["l216", "default", "l430"]):
             pl.set_subbatches(n)
             for _ in range(3):
                 pl.tick()
-            row.append("%d: %.4f" % (n, timed(pl.tick)))
+            row.append("%d: %.4f" % (n, sorted(timed_ms(pl.tick) for _ in range(12))[6]))   # median
         print("%-8s B=%-6d tick ms by windows  %s" % (tag, batch, "  ".join(row)), file=sys.__stdout__, flush=True)

@@ -10,18 +10,12 @@ if len(sys.argv) > 2 and sys.argv[1] == "--child":
     tag = sys.argv[3]
     import torch, bench
     from graphbasedlocaltrajectoryplanner_b200.planner import BatchPlanner
+    from tools.workload import timed_ms
     pl = BatchPlanner(bench.get_lattice(tag), device="cuda:0")
     pl.set_vel_params(**bench.vel_kwargs())
     pl.stage_scenarios(bench.make_batch(tag, int(os.environ.get("TUNE_BATCH", "10000")))); pl.upload(); pl.set_startpos()
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
-    st = torch.cuda.current_stream()
     def timed(fn, steps=10):
-        tot = 0.0
-        for _ in range(steps):
-            flush.fill_(1)
-            e0 = torch.cuda.Event(enable_timing=True); e1 = torch.cuda.Event(enable_timing=True)
-            e0.record(st); fn(); e1.record(st); torch.cuda.synchronize(); tot += e0.elapsed_time(e1)
-        return tot / steps
+        return sum(timed_ms(fn) for _ in range(steps)) / steps
     for _ in range(3): pl.tick()
     res = {"tick_ms": timed(pl.tick)}
     for stage, name in {1: "k_plan", 2: "k_path", 3: "k_vel"}.items():
