@@ -309,6 +309,12 @@ class Graph_LTPL(object):
         pl.upload()
         pl.set_startpos()
 
+    def set_gg_map(self, ax=None, ay=None, x0: float = 0.0, y0: float = 0.0, cell: float = 1.0) -> None:
+        """friction map of the track surface for the batched API (calc_vel_profile_batch, plan_batch, plan_stream):
+        ``BatchPlanner.set_gg_map``.  The single-scenario calc_vel_profile takes its local_gg argument as the reference
+        does and clears the map."""
+        self.planner.set_gg_map(ax, ay, x0, y0, cell)
+
     def calc_paths_batch(self) -> None:
         self.planner.calc_paths()
 

@@ -12,7 +12,7 @@ import os
 import subprocess
 import sys
 
-ABI_VERSION = 17
+ABI_VERSION = 18
 MAX_SUB = 8
 NSLOT = 3
 MAX_AXM = 32
@@ -65,7 +65,9 @@ class Params(C.Structure):
                 ("safety_d", C.c_double), ("n_axm", C.c_int32), ("traj_base_id", C.c_int32),
                 ("incl_emerg_traj", C.c_int32), ("filt_window", C.c_int32), ("delaycomp", C.c_double),
                 ("w_last_edges", C.c_double * 4),
-                ("axm_v", C.c_double * MAX_AXM), ("axm_a", C.c_double * MAX_AXM), ("axm_s", C.c_double * MAX_AXM)]
+                ("axm_v", C.c_double * MAX_AXM), ("axm_a", C.c_double * MAX_AXM), ("axm_s", C.c_double * MAX_AXM),
+                ("gg_map_x0", C.c_double), ("gg_map_y0", C.c_double), ("gg_map_inv_cell", C.c_double),
+                ("gg_map_nx", C.c_int32), ("gg_map_ny", C.c_int32)]
 
 
 class Dims(C.Structure):
@@ -80,7 +82,7 @@ BUFFER_FIELDS = ("pos", "heading", "vel", "vel_est", "n_obj", "obj", "sc_flags",
                  "n_pred", "prev_path", "prev_path_len", "prev_node_idx", "prev_nodes", "prev_n_nodes", "prev_coeff",
                  "prev_s_vx_ax", "prev_action_id", "prev_traj_len", "prev_trim", "sel_action", "pos_last", "t_const",
                  "st_info", "trim", "vel_plan", "course", "obj_dist", "zone_s0", "em_vx", "prev_em_vx", "prev_em_info",
-                 "gg", "prev_gg", "restart")
+                 "gg", "prev_gg", "restart", "gg_map")
 STATE_FIELDS = BUFFER_FIELDS[BUFFER_FIELDS.index("prev_path"):]   # NULL unless a stateful tick is planned
 
 

@@ -3,6 +3,7 @@
 //
 // build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -fmad=false -shared -Xcompiler -fPIC
 #include <atomic>
+#include <cmath>
 #include <cstddef>
 #include <cstdio>
 #include <cstdlib>
@@ -19,6 +20,7 @@
 #include "ltpl_emerg.cuh"
 #include "ltpl_state.cuh"
 #include "ltpl_smooth.cuh"
+#include "ltpl_gg_map.cuh"
 
 // the memory records are the int32 arrays BatchPlanner allocates: st_info [B][8], trim [NSLOT*B][4]
 static_assert(sizeof(LtplStateInfo) == 8 * sizeof(int32_t) && alignof(LtplStateInfo) == alignof(int32_t), "st_info row");
@@ -407,6 +409,18 @@ static int validate(const LtplLattice* lat, const LtplParams* prm, const LtplDim
     if (prm->filt_window < 0 || (prm->filt_window > 1 && prm->filt_window % 2 == 0))   // tph.conv_filt input check
         return fail("params.filt_window: window width of moving average filter must be odd (0 or 1: no smoothing)");
     if (prm->incl_emerg_traj && !bf->em_info) return fail("params.incl_emerg_traj needs buffers.em_info");
+    if (bf->gg_map) {   // the friction map fills the caller's gg planes (k_gg_map)
+        if (!bf->gg) return fail("buffers.gg_map needs buffers.gg: the planes the map is evaluated into");
+        if (reinterpret_cast<uintptr_t>(bf->gg_map) % 16 != 0)
+            return fail("buffers.gg_map must be 16-byte aligned (k_gg_map reads one ax, ay pair per 16-byte load)");
+        if (prm->gg_map_nx < 2 || prm->gg_map_ny < 2) return fail("params.gg_map_nx and params.gg_map_ny must be >= 2");
+        if ((int64_t)prm->gg_map_nx * prm->gg_map_ny > INT32_MAX)
+            return fail("params.gg_map_nx * params.gg_map_ny exceeds 32-bit indexing");
+        if (!std::isfinite(prm->gg_map_inv_cell) || !(prm->gg_map_inv_cell > 0.0))
+            return fail("params.gg_map_inv_cell must be finite and > 0");
+        if (!std::isfinite(prm->gg_map_x0) || !std::isfinite(prm->gg_map_y0))
+            return fail("params.gg_map_x0 and params.gg_map_y0 must be finite");
+    }
     if (!stateful) return 0;
     if (!bf->prev_path || !bf->prev_path_len || !bf->prev_node_idx || !bf->prev_nodes || !bf->prev_n_nodes ||
         !bf->prev_coeff || !bf->prev_s_vx_ax || !bf->prev_action_id || !bf->prev_traj_len || !bf->prev_trim ||
@@ -473,11 +487,16 @@ static int paths_window(const LtplLattice* lat, const LtplParams* prm, const Ltp
     return launch_k_path(lat, prm, w, bf, st, stateful);
 }
 
-// one scenario window of calc_vel_profile.  First tick: k_vel_res (exports its rows itself) (-> k_smooth) (-> k_emergency).
-// Stateful tick: k_ref -> k_vel_res -> k_backup -> k_prefix (-> k_smooth) -> k_export (-> k_emergency)
+// one scenario window of calc_vel_profile, behind k_gg_map when a friction map is set.  First tick: k_vel_res (exports its
+// rows itself) (-> k_smooth) (-> k_emergency).  Stateful tick: k_ref -> k_vel_res -> k_backup -> k_prefix (-> k_smooth) ->
+// k_export (-> k_emergency)
 static int vel_window(const LtplLattice* lat, const LtplParams* prm, const LtplDims* w, const LtplBuffers* bf,
                       cudaStream_t st, bool stateful) {
     const bool smooth = prm->filt_window > 1;
+    if (bf->gg_map) {
+        k_gg_map<<<ctas(LTPL_NSLOT * w->sub_cnt), kThreads, 0, st>>>(*prm, *w, *bf);
+        if (int r = check_launch("k_gg_map")) return r;
+    }
     if (stateful) {
         k_ref<<<ctas(w->sub_cnt), kThreads, 0, st>>>(lat->d, *prm, *w, *bf);
         if (int r = check_launch("k_ref")) return r;

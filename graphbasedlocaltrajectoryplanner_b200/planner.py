@@ -71,6 +71,32 @@ def read_online_config(path: str) -> dict:
                 delaycomp=cfg.getfloat('DELAY', 'delaycomp'))
 
 
+def check_gg_map(ax, ay, x0, y0, cell):
+    """input checks of a friction map (BatchPlanner.set_gg_map): ``ax``, ``ay`` 2-D [ny][nx] arrays (NumPy or torch) of
+    equal shape with ny, nx >= 2 and finite values > 0; ``x0``, ``y0`` finite; ``cell`` finite and > 0.  Raises
+    ValueError; returns (nx, ny, inv_cell) with inv_cell = 1 / cell in float64."""
+    shape_x, shape_y = tuple(ax.shape), tuple(ay.shape)
+    if shape_x != shape_y or len(shape_x) != 2:
+        raise ValueError("gg map: ax and ay must be 2-D arrays [ny][nx] of equal shape, got %s and %s"
+                         % (shape_x, shape_y))
+    ny, nx = shape_x
+    if nx < 2 or ny < 2:
+        raise ValueError("gg map: at least 2 x 2 vertices, got %d x %d" % (nx, ny))
+    if nx * ny > 2 ** 31 - 1:
+        raise ValueError("gg map: %d x %d vertices exceed 32-bit indexing" % (nx, ny))
+    for name, a in (("ax", ax), ("ay", ay)):
+        ok = bool(torch.all(torch.isfinite(a) & (a > 0))) if isinstance(a, torch.Tensor) \
+            else bool(np.all(np.isfinite(a) & (a > 0)))
+        if not ok:
+            raise ValueError("gg map: every %s value must be finite and > 0" % name)
+    x0, y0, cell = float(x0), float(y0), float(cell)
+    if not (np.isfinite(x0) and np.isfinite(y0)):
+        raise ValueError("gg map: the origin (x0, y0) must be finite")
+    if not (np.isfinite(cell) and cell > 0.0):
+        raise ValueError("gg map: cell must be finite and > 0, got %r" % cell)
+    return nx, ny, 1.0 / cell
+
+
 DEFAULT_ONLINE = dict(max_heading_offset=0.8, nmbr_export_points=115, v_max_offset=0.1, max_solutions=1,
                       filt_window_width=1, w_last_edges=[0.0, 0.5, 0.8], controller_type="PD",
                       control_params={"c_p": 1.25, "k_d": 0.025, "k_p": 0.2}, delaycomp=0.1)
@@ -123,6 +149,10 @@ class BatchPlanner(object):
         self.t = {}
         self.params = capi.Params()
         self._tick_count = 0
+        self._gg_map = None           # device [ny][nx][2] friction map of set_gg_map, or None
+        # whether the velocity half of the last tick ran with gg planes (uploaded or from the map): decides whether the
+        # next stateful tick brakes on its backup plan with those planes (prev_gg) or with the constant tuple
+        self._gg_planes_used = False
         self.on_device_start = None   # optional callable, called where a stateful tick's host staging ends (timing)
         self.set_vel_params()
 
@@ -278,6 +308,7 @@ class BatchPlanner(object):
             if name not in capi.STATE_FIELDS and name in t:   # `trim` is a state field: NULL unless the planner is stateful
                 setattr(buf, name, t[name].data_ptr())
         self.t, self.buf, self.dims = t, buf, d
+        self._gg_planes_used = False
         self._alloc_inputs(B, k_obj, k_pred)
         self._state = None   # buffers of the stateful tick, allocated by next_tick()
         # further compact export buffers: the pipelined stream planner lets the D2H of step i overlap step i + 1
@@ -295,15 +326,18 @@ class BatchPlanner(object):
         self._row_bytes = NE * 7 * 4
         if self._stateful:
             self._alloc_state()   # incl. zone_s0, which the FIRST tick has to fill
+        self._bind_gg_map()
 
     def set_local_gg_planes(self, ax=None, ay=None) -> None:
         """location dependent friction (calc_vel_profile(local_gg={action: [ndarray(P, 2)]}), OTH:649-666) for the batch:
         ``ax``, ``ay`` [NSLOT][B][P] (P <= p_max) = longitudinal / lateral limit at every point of every path (slot 0:
         straight | follow, 1: left, 2: right), aligned with the paths of the last calc_paths; None: back to the constant
-        tuple of set_vel_params().  The values are taken without gg_scale (VPFB:213-214 applies it)."""
+        tuple of set_vel_params().  The values are taken without gg_scale (VPFB:213-214 applies it).  Clears the friction
+        map of set_gg_map()."""
+        self._gg_map = None
+        self.buf.gg_map = None
         if ax is None:
             self.buf.gg = None
-            self._gg_active = False
             return
         ax = np.asarray(ax, dtype=np.float64)
         ay = np.asarray(ay, dtype=np.float64)
@@ -317,7 +351,47 @@ class BatchPlanner(object):
         host[1, :, :ay.shape[2]] = ay.reshape(NSLOT * B, -1)
         self.t["gg"].copy_(torch.from_numpy(host))
         self.buf.gg = self.t["gg"].data_ptr()
-        self._gg_active = True
+
+    def set_gg_map(self, ax=None, ay=None, x0: float = 0.0, y0: float = 0.0, cell: float = 1.0) -> None:
+        """location dependent friction from a map of the track surface, for the whole batch: ``ax``, ``ay`` [ny][nx] =
+        longitudinal / lateral limit (without gg_scale, like the local_gg rows) at the vertices of a regular grid with
+        vertex [0][0] at (x0, y0) and spacing ``cell`` metres.  NumPy arrays or torch tensors on this planner's device.
+        From now on the velocity half of every tick (tick, calc_vel_profile, next_tick, next_calc_vel_profile,
+        plan_stream) evaluates the map on the device along every planned path (bilinear, clamped to the grid; DESIGN.md
+        section 7), as calc_vel_profile(local_gg={action: [map(path[:, 0:2])]}) would take it.  The map is uploaded once
+        and stays until it is changed.  None: back to the constant tuple of set_vel_params().  Clears the planes of
+        set_local_gg_planes().  Bad input raises ValueError and changes nothing."""
+        if ax is None:
+            self._gg_map = None
+            if self.buf is not None:
+                self.buf.gg_map = None
+                self.buf.gg = None
+            return
+        for a in (ax, ay):
+            if isinstance(a, torch.Tensor) and a.device != self.device:
+                raise ValueError("gg map: a torch tensor must be on the planner's device %s, got %s" % (self.device,
+                                                                                                     a.device))
+        if not isinstance(ax, torch.Tensor):
+            ax = np.asarray(ax, dtype=np.float64)
+        if not isinstance(ay, torch.Tensor):
+            ay = np.asarray(ay, dtype=np.float64)
+        nx, ny, inv_cell = check_gg_map(ax, ay, x0, y0, cell)
+        dev = lambda a: torch.as_tensor(a, dtype=torch.float64).to(self.device)   # noqa: E731
+        self._gg_map = torch.stack((dev(ax), dev(ay)), dim=-1).contiguous()   # [ny][nx][2]: one 16-byte load per vertex
+        p = self.params
+        p.gg_map_x0, p.gg_map_y0, p.gg_map_inv_cell = float(x0), float(y0), inv_cell
+        p.gg_map_nx, p.gg_map_ny = nx, ny
+        self._bind_gg_map()
+
+    def _bind_gg_map(self) -> None:
+        """buffers.gg_map and the gg planes the library fills from it (allocated with the other buffers)"""
+        if self._gg_map is None or self.buf is None:
+            return
+        if "gg" not in self.t:
+            self.t["gg"] = torch.ones((2, NSLOT * self.dims.batch, self.dims.p_max), dtype=torch.float64,
+                                      device=self.device)
+        self.buf.gg = self.t["gg"].data_ptr()
+        self.buf.gg_map = self._gg_map.data_ptr()
 
     def device_bytes(self) -> int:
         return int(sum(v.numel() * v.element_size() for v in self.t.values()) + self.blob.numel())
@@ -507,6 +581,7 @@ class BatchPlanner(object):
         self._tick_count += 1
         self.params.traj_base_id = 10 * self._tick_count
         self._call(name)
+        self._gg_planes_used = self.buf.gg is not None
 
     def set_startpos(self) -> None:
         self._call("ltpl_set_startpos_batch")
@@ -593,15 +668,15 @@ class BatchPlanner(object):
         for k in self._SMALL:
             setattr(buf, "prev_" + k, st["prev_small"][k].data_ptr())
         # location dependent local_gg of the last tick = backup for a brake on the old plan (__backup_path_gg, OTH:970)
-        if getattr(self, "_gg_active", False):
+        if self._gg_planes_used:
             if "gg" not in st["other"]:
                 st["other"]["gg"] = torch.ones_like(t["gg"])
             t["gg"], st["other"]["gg"] = st["other"]["gg"], t["gg"]
             buf.prev_gg = st["other"]["gg"].data_ptr()
         else:
             buf.prev_gg = None
-        buf.gg = None            # this tick's local_gg arrives with its calc_vel_profile
-        self._gg_active = False
+        buf.gg = None            # this tick's local_gg arrives with its calc_vel_profile ...
+        self._bind_gg_map()      # ... or from the friction map, into this tick's planes
         # a zone under a NEW id is a new zone object: its unblock window is evaluated at this tick (OLI:155-237, GLNT:43-77)
         zkey = sc.zone_key if sc.zone_key is not None else np.zeros(sc.size, dtype=np.int64)
         last = getattr(self, "_zone_key", None)               # of the batch staged for the previous tick

@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define LTPL_ABI_VERSION 17
+#define LTPL_ABI_VERSION 18
 
 /* action ids (OTH:14-17 ACTION_ID_MAP) */
 #define LTPL_ACT_NONE (-1)
@@ -168,6 +168,11 @@ typedef struct LtplParams {
     double axm_v[LTPL_MAX_AXM];
     double axm_a[LTPL_MAX_AXM];
     double axm_s[LTPL_MAX_AXM];  /* slopes (a[i+1] - a[i]) / (v[i+1] - v[i]) exactly as np.interp forms them  */
+    /* friction map (buffers.gg_map; unused while it is NULL): a regular grid of gg_map_nx x gg_map_ny vertices, vertex   */
+    /* [0][0] at (gg_map_x0, gg_map_y0), spacing 1 / gg_map_inv_cell in x and y (DESIGN.md section 7)                    */
+    double gg_map_x0, gg_map_y0; /* finite                                                                            */
+    double gg_map_inv_cell;      /* 1 / cell in float64, finite and > 0                                               */
+    int32_t gg_map_nx, gg_map_ny; /* >= 2 each, nx * ny < 2^31                                                        */
 } LtplParams;
 
 /* capacities chosen by the host from the lattice (see lattice_blob.py: capacities()) */
@@ -299,8 +304,9 @@ typedef struct LtplBuffers {
     const double* prev_em_vx;       /* [B][n_export] the previous tick's                                                   */
     const int32_t* prev_em_info;    /* [B][3] the previous tick's em_info (all -1 when it had no emergency trajectory)     */
     /* location dependent friction: calc_vel_profile(local_gg={action: [ndarray(P, 2)]}) (OTH:649-666, VPFB:194-227).     */
-    /* NULL: the constant params.gg_ax / gg_ay of the tuple form.  Rows are aligned with the path planes.                 */
-    const double* gg;               /* [2][NSLOT*B][p_max] planes ax_max, ay_max per path point (without gg_scale)         */
+    /* NULL: the constant params.gg_ax / gg_ay of the tuple form.  Rows are aligned with the path planes.  Written by the  */
+    /* library (points [0, path_len) of every path) when gg_map is set, read only otherwise.                             */
+    double* gg;                     /* [2][NSLOT*B][p_max] planes ax_max, ay_max per path point (without gg_scale)         */
     const double* prev_gg;          /* the previous tick's `gg` (brake on the backup plan, OTH:970-975); NULL: constant     */
     /* restart of single scenarios inside a stateful tick: Graph_LTPL.set_startpos on a live instance (OTH:161-179, 204:   */
     /* reinit_iterative_memory).  Read by ltpl_next_calc_paths_batch and ltpl_next_tick_batch only; NULL: no restarts.     */
@@ -308,6 +314,10 @@ typedef struct LtplBuffers {
     /* vel (in-track and heading checks, forced 'straight' constant segment, cut 0, profile from vel, no backup plan); its */
     /* zone is processed anew.  Trajectory ids keep counting.  t_const and sel_action of the scenario are ignored.         */
     const int32_t* restart;         /* [B] non-zero: set_startpos for this scenario inside the stateful tick               */
+    /* friction map of the whole batch (geometry in params.gg_map_*): the velocity half of every tick fills `gg` with its   */
+    /* bilinear interpolation at every path point (k_gg_map, DESIGN.md section 7) -- calc_vel_profile(local_gg={action:    */
+    /* [map(path[:, 0:2])]}).  Needs `gg` and 16-byte alignment.  NULL: `gg` is read as the caller left it.               */
+    const double* gg_map;           /* [ny][nx][2] ax_max, ay_max per vertex (without gg_scale), one 16-byte pair each     */
 } LtplBuffers;
 
 /* stand-alone forward/backward ggv velocity profile over dense path arrays (BASELINE.json config 5).                   */

@@ -53,6 +53,18 @@ sel = pr.t["action_id"].max(dim=0).values.clamp(min=0).cpu().numpy()
 pr.next_tick(sc, sel_action=sel, t_const=0.1)
 r = pr.records()
 print("stateful tick after restarts, trajectories:", sum(len(x.get("traj", {})) for x in r))
+# a friction map over part of the track (k_gg_map in front of the velocity kernels), emergency trajectory on: a first
+# tick and a stateful tick (the backup brake reads the last tick's map planes)
+from tests import gg_map_ref as M
+ax, ay = M.surface_map(3.7, x0=-300.0, y0=-150.0, width=500.0, height=350.0)
+pm = BatchPlanner(H.lattice_for("default"), device="cuda:0", stateful=True)
+pm.set_vel_params(ax_max_machines=g["ax_max_machines"], incl_emerg_traj=True, **VEL)
+pm.set_gg_map(ax, ay, -300.0, -150.0, 3.7)
+pm.stage_scenarios(sc); pm.upload(); pm.set_startpos(); pm.tick()
+sel = pm.t["action_id"].max(dim=0).values.clamp(min=0).cpu().numpy()
+pm.next_tick(sc, sel_action=sel, t_const=0.1)
+r = pm.records()
+print("friction map stateful tick, trajectories:", sum(len(x.get("traj", {})) for x in r))
 mb =make_velocity_microbench(200, 150, seed=3)
 vx, ax = calc_vel_profile_batch(pl, mb["kappa"], mb["el"], mb["v_start"], mb["v_end"])
 print("dense vx mean", float(np.mean(vx)))
