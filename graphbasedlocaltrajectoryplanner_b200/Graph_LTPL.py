@@ -303,7 +303,8 @@ class Graph_LTPL(object):
     # ------------------------------------------------------------------------------------------------------------------
     # batched API
     # ------------------------------------------------------------------------------------------------------------------
-    def set_startpos_batch(self, scenarios: ScenarioBatch, vel_est=None) -> None:
+    def set_startpos_batch(self, scenarios, vel_est=None) -> None:
+        """set_startpos for a ScenarioBatch, or for a DeviceScenarioBatch staged on the device without host staging"""
         pl = self.planner
         pl.stage_scenarios(scenarios, vel_est=vel_est)
         pl.upload()
@@ -325,12 +326,13 @@ class Graph_LTPL(object):
         pl.calc_vel_profile()
         return pl.download()
 
-    def plan_batch(self, scenarios: ScenarioBatch = None, synchronize: bool = True) -> dict:
+    def plan_batch(self, scenarios=None, synchronize: bool = True) -> dict:
         """One end-to-end batched tick: host scenario arrays -> (H2D) -> set_startpos -> calc_paths -> calc_vel_profile
         -> (D2H) -> pinned host action sets: ``traj`` [n_rows][n_export][7] fp32 (compact: one row per kept
         trajectory), ``exp_q`` (row -> path id q = slot * B + b), ``traj_row`` [NSLOT][B] (path -> row or -1),
         ``traj_len``, ``traj_id``, ``action_id``, ``status``, ``sc_flags``, ``n_rows``.
-        With ``scenarios=None`` the previously staged batch is planned again."""
+        With ``scenarios=None`` the previously staged batch is planned again.  A DeviceScenarioBatch skips the host
+        staging and the H2D copy (BatchPlanner.stage_scenarios); the results are downloaded all the same."""
         pl = self.planner
         if scenarios is not None:
             pl.stage_scenarios(scenarios)

@@ -12,7 +12,7 @@ import os
 import subprocess
 import sys
 
-ABI_VERSION = 18
+ABI_VERSION = 19
 MAX_SUB = 8
 NSLOT = 3
 MAX_AXM = 32
@@ -95,10 +95,23 @@ class VelBatch(C.Structure):
                 ("v_start", C.c_void_p), ("v_end", C.c_void_p), ("vx", C.c_void_p), ("ax", C.c_void_p)]
 
 
+class StageSrc(C.Structure):
+    _fields_ = [("pos", C.c_void_p), ("pos_s", C.c_int64 * 2), ("heading", C.c_void_p), ("heading_s", C.c_int64),
+                ("vel", C.c_void_p), ("vel_s", C.c_int64), ("vel_est", C.c_void_p), ("vel_est_s", C.c_int64),
+                ("n_obj", C.c_void_p), ("n_obj_s", C.c_int64), ("obj", C.c_void_p), ("obj_s", C.c_int64 * 3),
+                ("pred", C.c_void_p), ("pred_s", C.c_int64 * 4), ("n_pred", C.c_void_p), ("n_pred_s", C.c_int64 * 2),
+                ("zone_sel", C.c_void_p), ("zone_sel_s", C.c_int64), ("zone_key", C.c_void_p), ("zone_key_s", C.c_int64),
+                ("zone_key_last", C.c_void_p), ("sel_action", C.c_void_p), ("sel_action_s", C.c_int64),
+                ("t_const", C.c_void_p), ("t_const_s", C.c_int64), ("restart", C.c_void_p), ("restart_s", C.c_int64),
+                ("t_const_value", C.c_double), ("k_src", C.c_int32), ("kp_src", C.c_int32), ("kp_dst", C.c_int32),
+                ("sel_action_bytes", C.c_int32), ("restart_bytes", C.c_int32), ("zone_key_rule", C.c_int32)]
+
+
 EXPORTS = ("ltpl_version", "ltpl_last_error", "ltpl_sizeof", "ltpl_max_objects", "ltpl_lattice_create",
            "ltpl_lattice_destroy", "ltpl_set_startpos_batch", "ltpl_calc_paths_batch", "ltpl_calc_vel_profile_batch",
            "ltpl_tick_batch", "ltpl_velprofile_batch", "ltpl_launch_count", "ltpl_launch_stage", "ltpl_next_tick_batch",
-           "ltpl_next_calc_paths_batch", "ltpl_next_calc_vel_profile_batch", "ltpl_set_subbatches")
+           "ltpl_next_calc_paths_batch", "ltpl_next_calc_vel_profile_batch", "ltpl_set_subbatches",
+           "ltpl_stage_inputs_batch")
 
 
 def build_library(verbose: bool = False) -> str:
@@ -154,9 +167,11 @@ def load_library():
     lib.ltpl_launch_stage.restype = C.c_int
     lib.ltpl_velprofile_batch.argtypes = [C.POINTER(Params), C.POINTER(VelBatch), C.c_void_p]
     lib.ltpl_velprofile_batch.restype = C.c_int
+    lib.ltpl_stage_inputs_batch.argtypes = [C.POINTER(Dims), C.POINTER(Buffers), C.POINTER(StageSrc), C.c_void_p]
+    lib.ltpl_stage_inputs_batch.restype = C.c_int
     if lib.ltpl_version() != ABI_VERSION:
         raise RuntimeError("libltpl_b200.so ABI version %d != binding %d" % (lib.ltpl_version(), ABI_VERSION))
-    for which, st in enumerate((LatticeHeader, Params, Dims, Buffers, VelBatch)):
+    for which, st in enumerate((LatticeHeader, Params, Dims, Buffers, VelBatch, StageSrc)):
         if lib.ltpl_sizeof(which) != C.sizeof(st):
             raise RuntimeError("ctypes mirror of %s has %d bytes, library says %d" % (st.__name__, C.sizeof(st),
                                                                                       lib.ltpl_sizeof(which)))

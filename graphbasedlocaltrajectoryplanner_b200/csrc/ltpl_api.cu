@@ -21,6 +21,7 @@
 #include "ltpl_state.cuh"
 #include "ltpl_smooth.cuh"
 #include "ltpl_gg_map.cuh"
+#include "ltpl_stage.cuh"
 
 // the memory records are the int32 arrays BatchPlanner allocates: st_info [B][8], trim [NSLOT*B][4]
 static_assert(sizeof(LtplStateInfo) == 8 * sizeof(int32_t) && alignof(LtplStateInfo) == alignof(int32_t), "st_info row");
@@ -187,6 +188,7 @@ int ltpl_sizeof(int which) {
         case 2: return (int)sizeof(LtplDims);
         case 3: return (int)sizeof(LtplBuffers);
         case 4: return (int)sizeof(LtplVelBatch);
+        case 5: return (int)sizeof(LtplStageSrc);
         default: return -1;
     }
 }
@@ -609,6 +611,27 @@ int ltpl_velprofile_batch(const LtplParams* prm, const LtplVelBatch* vb, void* s
     else
         k_velprofile<false><<<(vb->n_paths + 31) / 32, 32, VD_SMEM_BYTES, static_cast<cudaStream_t>(stream)>>>(*prm, *vb);
     return check_launch("k_velprofile");
+}
+
+int ltpl_stage_inputs_batch(const LtplDims* dm, const LtplBuffers* bf, const LtplStageSrc* src, void* stream) {
+    if (!dm || !bf || !src) return fail("null argument");
+    if (dm->batch <= 0 || dm->k_obj < 1) return fail("dims.batch and dims.k_obj must be > 0");
+    if (!bf->pos || !bf->heading || !bf->vel || !bf->vel_est || !bf->n_obj || !bf->obj || !bf->zone_sel || !bf->n_pred)
+        return fail("stage: buffers pos, heading, vel, vel_est, n_obj, obj, zone_sel and n_pred must be set");
+    if (!src->pos || !src->heading || !src->vel || !src->n_obj || (src->k_src > 0 && !src->obj))
+        return fail("stage: src.pos, src.heading, src.vel, src.n_obj and (k_src > 0) src.obj must be set");
+    if (src->k_src < 0 || src->k_src > dm->k_obj) return fail("stage: src.k_src must be in [0, dims.k_obj]");
+    if (src->kp_dst < 0 || (src->kp_dst > 0 && !bf->obj_pred)) return fail("stage: src.kp_dst > 0 needs buffers.obj_pred");
+    if (src->pred && (!src->n_pred || src->kp_src < 0 || src->kp_src > src->kp_dst))
+        return fail("stage: src.pred needs src.n_pred and src.kp_src in [0, kp_dst]");
+    if (src->sel_action && (!bf->sel_action || !bf->t_const || (src->sel_action_bytes != 4 && src->sel_action_bytes != 8)))
+        return fail("stage: src.sel_action needs buffers.sel_action, buffers.t_const and sel_action_bytes 4 or 8");
+    if (src->restart && (!bf->restart || (src->restart_bytes != 1 && src->restart_bytes != 4 && src->restart_bytes != 8)))
+        return fail("stage: src.restart needs buffers.restart and restart_bytes 1, 4 or 8");
+    if (src->zone_key_rule && (!src->zone_key_last || !bf->zone_s0))
+        return fail("stage: src.zone_key_rule needs src.zone_key_last and buffers.zone_s0");
+    k_stage<<<ctas(dm->batch), kThreads, 0, static_cast<cudaStream_t>(stream)>>>(*dm, *bf, *src);
+    return check_launch("k_stage");
 }
 
 #ifdef LTPL_PROFILE_PHASES

@@ -21,7 +21,7 @@ import torch
 from . import capi
 from .lattice import Lattice
 from .lattice_blob import pack_lattice
-from .scenarios import ScenarioBatch
+from .scenarios import DeviceScenarioBatch, ScenarioBatch
 
 NSLOT = capi.NSLOT
 
@@ -154,6 +154,9 @@ class BatchPlanner(object):
         # next stateful tick brakes on its backup plan with those planes (prev_gg) or with the constant tuple
         self._gg_planes_used = False
         self.on_device_start = None   # optional callable, called where a stateful tick's host staging ends (timing)
+        self._staged_on_device = False   # the last staged batch was a DeviceScenarioBatch: upload() has nothing to copy
+        self._zones_dev = None        # the zone list whose bitmasks the device path uploaded last (None: none / stale)
+        self._zone_key_dev = None     # [B] int64: zone keys of the last device staging (k_stage reads and writes it)
         self.set_vel_params()
 
     def __del__(self):
@@ -309,6 +312,7 @@ class BatchPlanner(object):
                 setattr(buf, name, t[name].data_ptr())
         self.t, self.buf, self.dims = t, buf, d
         self._gg_planes_used = False
+        self._zones_dev = None
         self._alloc_inputs(B, k_obj, k_pred)
         self._state = None   # buffers of the stateful tick, allocated by next_tick()
         # further compact export buffers: the pipelined stream planner lets the D2H of step i overlap step i + 1
@@ -410,8 +414,17 @@ class BatchPlanner(object):
         rows = self.h_out["traj"].shape[0] if n_rows is None else n_rows
         return int(meta + rows * self._row_bytes)
 
-    def stage_scenarios(self, sc: ScenarioBatch, vel_est=None, which: int = 0) -> None:
-        """copy a scenario batch into the pinned staging buffers (host memcpy)."""
+    def stage_scenarios(self, sc, vel_est=None, which: int = 0) -> None:
+        """copy a scenario batch into the pinned staging buffers (host memcpy).  A DeviceScenarioBatch is written into
+        the device inputs instead, by one kernel on the current stream (k_stage, no host synchronisation unless the
+        batch brings more object slots or prediction points than allocated); upload() then has nothing to copy.
+        ``vel_est`` may then be a device tensor [B]."""
+        if isinstance(sc, DeviceScenarioBatch):
+            vel_est = self._device_args(sc, vel_est)[0]
+            self._grow_for(sc)
+            self._stage_device(sc, vel_est)
+            return
+        self._staged_on_device = False
         kp = 0 if sc.pred is None else int(sc.pred.shape[2])
         if self.dims is None or sc.size != self.dims.batch or sc.obj.shape[1] > self.dims.k_obj or kp > self._k_pred_cap:
             self.allocate(sc.size, sc.obj.shape[1], kp)
@@ -441,9 +454,16 @@ class BatchPlanner(object):
 
     def _upload_zones(self, zones) -> None:
         """zone bitmasks: bit (node_off[layer] + node) of mask z = that node is blocked by zone z (GLNT:46, 96-99)."""
+        self._zones_dev = None
         if not zones:
             self.dims.n_zones = 0
             return
+        self.t["zone_bits"] = torch.from_numpy(self._zone_bits(zones)).to(self.device)
+        self.buf.zone_bits = self.t["zone_bits"].data_ptr()
+        self.dims.n_zones = len(zones)
+
+    def _zone_bits(self, zones) -> np.ndarray:
+        """the int32 [n_zones][n_zone_words] bitmasks of a zone list; ValueError for ids outside the lattice"""
         w = int(self.dims.n_zone_words)
         bits = np.zeros((len(zones), w), dtype=np.uint32)
         for z, (lay, nod) in enumerate(zones):
@@ -453,11 +473,108 @@ class BatchPlanner(object):
             if lay.size and (np.any(nod < 0) or np.any(g >= self.node_off[lay + 1])):
                 raise ValueError("zone node id outside its layer")
             np.bitwise_or.at(bits[z], g >> 5, (np.uint32(1) << (g & 31).astype(np.uint32)))
-        self.t["zone_bits"] = torch.from_numpy(bits.view(np.int32)).to(self.device)
-        self.buf.zone_bits = self.t["zone_bits"].data_ptr()
+        return bits.view(np.int32)
+
+    # -- scenario inputs from device tensors (DeviceScenarioBatch -> k_stage) ----------------------------------------------
+    def _device_args(self, sc: DeviceScenarioBatch, vel_est=None, sel_action=None, t_const=None, restart=None):
+        """checks of a device batch and of the per-scenario arguments of its tick, from shapes, dtypes and devices only
+        (no values, no synchronisation): ValueError before anything launches.  Returns vel_est, sel_action, t_const,
+        restart as device tensors [B] or None; t_const may also come back as a float (broadcast by k_stage).  Host
+        arrays are accepted and uploaded here (a synchronous copy)."""
+        sc.check(self.device)
+        check_object_count(sc.obj.shape[1], self.max_objects)
+        B, dev = sc.size, sc.pos.device
+
+        def arg(name, a, dtypes, np_dt):
+            if a is None:
+                return None
+            if not isinstance(a, torch.Tensor):
+                try:
+                    a = np.broadcast_to(np.asarray(a, dtype=np_dt), (B,))
+                except ValueError:
+                    raise ValueError("%s must broadcast to shape [%d]" % (name, B)) from None
+                return torch.as_tensor(np.ascontiguousarray(a)).to(dev)
+            if a.device != dev or a.dtype not in dtypes or tuple(a.shape) != (B,):
+                raise ValueError("%s must be a tensor [%d] of %s on %s, got %s %s on %s" % (
+                    name, B, " / ".join(str(d) for d in dtypes), dev, a.dtype, tuple(a.shape), a.device))
+            return a
+        if t_const is not None and not isinstance(t_const, torch.Tensor) and np.ndim(t_const) == 0:
+            t_const = float(t_const)
+        else:
+            t_const = arg("t_const", t_const, (torch.float64,), np.float64)
+        return (arg("vel_est", vel_est, (torch.float64,), np.float64),
+                arg("sel_action", sel_action, (torch.int32, torch.int64), np.int32), t_const,
+                arg("restart", restart, (torch.bool, torch.uint8, torch.int8, torch.int32, torch.int64), np.int32))
+
+    def _grow_for(self, sc: DeviceScenarioBatch) -> None:
+        """buffers for the batch size, object slots and prediction points of a device batch (see allocate: growing them
+        synchronises)"""
+        kp = 0 if sc.pred is None else int(sc.pred.shape[2])
+        if self.dims is None or sc.size != self.dims.batch or sc.obj.shape[1] > self.dims.k_obj or kp > self._k_pred_cap:
+            self.allocate(sc.size, sc.obj.shape[1], kp)
+
+    def _stage_device(self, sc: DeviceScenarioBatch, vel_est=None, sel_action=None, t_const=None, restart=None,
+                      zone_rule: bool = False) -> None:
+        """k_stage: the inputs of a device batch into the input set in use, with the bytes stage_scenarios + upload
+        write (and with sel_action those of _stage_next); zone_rule: the zone key rule of a stateful tick"""
+        src = capi.StageSrc()
+
+        def put(name, a):
+            if a is not None:
+                setattr(src, name, a.data_ptr())
+                stride = a.stride()
+                if isinstance(getattr(src, name + "_s"), int):
+                    setattr(src, name + "_s", stride[0])
+                else:
+                    getattr(src, name + "_s")[:] = stride[:len(getattr(src, name + "_s"))]
+        for name in ("pos", "heading", "vel", "n_obj", "obj", "zone_sel", "zone_key", "pred", "n_pred"):
+            put(name, getattr(sc, name))
+        put("vel_est", vel_est)
+        src.k_src = int(sc.obj.shape[1])
+        src.kp_src = 0 if sc.pred is None else int(sc.pred.shape[2])
+        src.kp_dst = self._k_pred_cap
+        self.dims.k_pred = 0 if sc.pred is None else self._k_pred_cap
+        if sel_action is not None:
+            put("sel_action", sel_action)
+            src.sel_action_bytes = sel_action.element_size()
+            if isinstance(t_const, torch.Tensor):
+                put("t_const", t_const)
+            else:
+                src.t_const_value = float(t_const)
+        if restart is not None:
+            put("restart", restart)
+            src.restart_bytes = restart.element_size()
+        # the zone key of the last staging lives on the device from now on; after a host staging it crosses over once
+        B = self.dims.batch
+        last = getattr(self, "_zone_key", None)
+        if self._zone_key_dev is None or self._zone_key_dev.shape[0] != B:
+            self._zone_key_dev = torch.zeros((B,), dtype=torch.int64, device=self.device)
+        if isinstance(last, np.ndarray) and last.shape == (B,):
+            self._zone_key_dev.copy_(torch.from_numpy(last))
+        src.zone_key_last = self._zone_key_dev.data_ptr()
+        src.zone_key_rule = int(zone_rule and last is not None and tuple(last.shape) == (B,))
+        self._zone_key = self._zone_key_dev
+        self._stage_zones_device(sc.zones)
+        self._staged_on_device = True
+        capi.check(self.lib, self.lib.ltpl_stage_inputs_batch(C.byref(self.dims), C.byref(self.buf), C.byref(src),
+                                                              self.stream), "ltpl_stage_inputs_batch")
+
+    def _stage_zones_device(self, zones) -> None:
+        """zone bitmasks of a device batch: uploaded (pinned, asynchronously) only when the zone list changed"""
+        if not zones:
+            self.dims.n_zones = 0
+            return
+        key = tuple((np.asarray(lay).tobytes(), np.asarray(nod).tobytes()) for lay, nod in zones)
+        if key != self._zones_dev:
+            bits = torch.from_numpy(self._zone_bits(zones)).pin_memory()
+            self.t["zone_bits"] = bits.to(self.device, non_blocking=True)
+            self.buf.zone_bits = self.t["zone_bits"].data_ptr()
+            self._zones_dev = key
         self.dims.n_zones = len(zones)
 
     def upload(self, which: int = 0) -> None:
+        if self._staged_on_device:   # k_stage has already written the device inputs
+            return
         self.d_in_raw.copy_(self.h_in_raw[which], non_blocking=True)      # one packed H2D copy
         ev = torch.cuda.Event()
         ev.record(torch.cuda.current_stream(self.device))
@@ -465,7 +582,20 @@ class BatchPlanner(object):
 
     def set_estimates(self, pos_est=None, vel_est=None) -> None:
         """position / velocity estimates of calc_vel_profile (LTPL:344-346) for the staged batch: written into the pinned
-        staging set 0 and copied to the device on the current stream."""
+        staging set 0 and copied to the device on the current stream.  Device tensors (float64 on the planner's device,
+        [B][2] / [B]) are copied on the stream without the host."""
+        for name, a in (("pos", pos_est), ("vel_est", vel_est)):
+            if isinstance(a, torch.Tensor):
+                if a.device != self.t[name].device or a.dtype != torch.float64 or a.numel() != self.t[name].numel():
+                    raise ValueError("%s: a float64 tensor of %d values on %s, got %s %s on %s" % (
+                        name, self.t[name].numel(), self.t[name].device, a.dtype, tuple(a.shape), a.device))
+        for name, a in (("pos", pos_est), ("vel_est", vel_est)):
+            if isinstance(a, torch.Tensor):
+                self.t[name].copy_(a.reshape(self.t[name].shape))
+        pos_est = None if isinstance(pos_est, torch.Tensor) else pos_est
+        vel_est = None if isinstance(vel_est, torch.Tensor) else vel_est
+        if pos_est is None and vel_est is None:
+            return
         if self._h2d_ev[0] is not None:
             self._h2d_ev[0].synchronize()
             self._h2d_ev[0] = None
@@ -550,6 +680,9 @@ class BatchPlanner(object):
                 j = inflight.pop(0)
                 ev_d2h[j].synchronize()
                 yield self.h_out_sets[j]
+            if isinstance(sc, DeviceScenarioBatch):
+                raise ValueError("plan_stream overlaps the host staging of ScenarioBatch objects; plan a "
+                                 "DeviceScenarioBatch with plan_batch or tick()")
             if device_hook is not None and hasattr(device_hook, "before"):
                 device_hook.before(k)   # e.g. wait until a collective that still reads buffer set k has finished
             self.stage_scenarios(sc, vel_est=vel_est, which=k)
@@ -635,10 +768,7 @@ class BatchPlanner(object):
             self.buf.restart = None
             return
         st = self._state
-        if "restart" not in st:
-            st["restart"] = torch.zeros((self.dims.batch,), dtype=torch.int32, device=self.device)
-            st["h_restart"] = torch.zeros((self.dims.batch,), dtype=torch.int32).pin_memory()
-            st["restart_ev"] = None
+        self._restart_buffer()
         if st["restart_ev"] is not None:      # the last copy may still read the pinned staging
             st["restart_ev"].synchronize()
         st["h_restart"].numpy()[...] = mask
@@ -647,15 +777,31 @@ class BatchPlanner(object):
         st["restart_ev"].record(torch.cuda.current_stream(self.device))
         self.buf.restart = st["restart"].data_ptr()
 
-    def _stage_next(self, sc: ScenarioBatch, sel_action, t_const, vel_est, restart=None) -> None:
+    def _restart_buffer(self) -> torch.Tensor:
+        """buffers.restart of the stateful tick ([B] int32 on the device) with its pinned staging"""
+        st = self._state
+        if "restart" not in st:
+            st["restart"] = torch.zeros((self.dims.batch,), dtype=torch.int32, device=self.device)
+            st["h_restart"] = torch.zeros((self.dims.batch,), dtype=torch.int32).pin_memory()
+            st["restart_ev"] = None
+        return st["restart"]
+
+    def _stage_next(self, sc, sel_action, t_const, vel_est, restart=None) -> None:
         """host side of a stateful tick: pointer swaps, the host memcpy into the pinned staging set, ONE packed H2D copy
         (scenario arrays incl. sel_action / t_const) and ONE device copy (the small per-path arrays of the last tick);
-        with restarts one more small H2D copy (the mask)."""
+        with restarts one more small H2D copy (the mask).  A DeviceScenarioBatch replaces the memcpy, the uploads and the
+        host zone-key comparison by one k_stage launch."""
         if sc.size != self.dims.batch:
             raise ValueError("stateful tick: the batch size must not change within a session (re-anchor with "
                              "set_startpos on a new batch, or restart single scenarios with `restart`)")
-        check_object_count(sc.obj.shape[1], self.max_objects)   # before the swaps below: a refused list changes nothing
-        mask = self._restart_mask(restart)                       # (likewise)
+        on_device = isinstance(sc, DeviceScenarioBatch)
+        if on_device:   # before the swaps below: refused inputs change nothing
+            if sel_action is None or t_const is None:
+                raise ValueError("stateful tick: sel_action and t_const are required")
+            dev_args = self._device_args(sc, vel_est, sel_action, t_const, restart)
+        else:
+            check_object_count(sc.obj.shape[1], self.max_objects)   # before the swaps below: a refused list changes nothing
+            mask = self._restart_mask(restart)                       # (likewise)
         if self._state is None:
             self._alloc_state()
         st, t, buf = self._state, self.t, self.buf
@@ -677,9 +823,14 @@ class BatchPlanner(object):
             buf.prev_gg = None
         buf.gg = None            # this tick's local_gg arrives with its calc_vel_profile ...
         self._bind_gg_map()      # ... or from the friction map, into this tick's planes
+        if on_device:
+            self._stage_next_device(sc, dev_args)
+            return
         # a zone under a NEW id is a new zone object: its unblock window is evaluated at this tick (OLI:155-237, GLNT:43-77)
         zkey = sc.zone_key if sc.zone_key is not None else np.zeros(sc.size, dtype=np.int64)
         last = getattr(self, "_zone_key", None)               # of the batch staged for the previous tick
+        if isinstance(last, torch.Tensor):                    # staged from a device batch: crosses over once
+            last = last.cpu().numpy()
         if last is not None and last.shape == zkey.shape:
             changed = np.nonzero((zkey != last) & (zkey != 0))[0]
             if changed.size:
@@ -701,6 +852,24 @@ class BatchPlanner(object):
         self.upload()
         self._stage_restart(mask)
 
+    def _stage_next_device(self, sc: DeviceScenarioBatch, dev_args) -> None:
+        """_stage_next of a device batch behind the swaps: the other input copy, then k_stage (inputs, sel_action,
+        t_const, restart mask and the zone key rule)"""
+        st, t, buf = self._state, self.t, self.buf
+        self._pos_last = t["pos"]
+        self._grow_for(sc)
+        self._use_inputs(1 - self._in_cur)
+        buf.pos_last = self._pos_last.data_ptr()
+        for k in ("st_info", "vel_plan", "course", "obj_dist"):
+            setattr(buf, k, st[k].data_ptr())
+        buf.sel_action = t["sel_action"].data_ptr()
+        buf.t_const = t["t_const"].data_ptr()
+        vel_est, sel_action, t_const, restart = dev_args
+        buf.restart = None if restart is None else self._restart_buffer().data_ptr()
+        if self.on_device_start is not None:
+            self.on_device_start()
+        self._stage_device(sc, vel_est, sel_action, t_const, restart, zone_rule=True)
+
     def next_calc_paths(self, sc: ScenarioBatch, sel_action, t_const, vel_est=None, restart=None) -> None:
         """calc_paths of a stateful tick (OTH:289-516 with the iterative memory): ``sc`` carries the object
         lists (its poses are only used by ``next_calc_vel_profile``), ``sel_action`` = action id (capi.ACT_*) every
@@ -709,7 +878,10 @@ class BatchPlanner(object):
         calc_vel_profile() after set_startpos(), or a stateful tick) must have run on this planner.
         ``restart``: boolean array [B]; a true entry restarts that scenario inside this tick, as set_startpos(sc.pos[b],
         sc.heading[b], sc.vel[b]) on a live planner followed by a first tick (its memory is dropped, its sel_action and
-        t_const are ignored); the other scenarios keep theirs.  A wrong shape raises ValueError and changes nothing."""
+        t_const are ignored); the other scenarios keep theirs.  A wrong shape raises ValueError and changes nothing.
+        With a DeviceScenarioBatch, ``sel_action`` (int32 / int64), ``t_const`` (float64 or a scalar), ``vel_est``
+        (float64) and ``restart`` (bool or integer) may be device tensors [B]; the tick then runs without a host
+        synchronisation (a mask tensor is passed to the library as it is, whether or not an entry is set)."""
         self._stage_next(sc, sel_action, t_const, vel_est, restart)
         self._call("ltpl_next_calc_paths_batch")
 
@@ -728,6 +900,20 @@ class BatchPlanner(object):
 
     def launch_count(self) -> int:
         return int(self.lib.ltpl_launch_count())
+
+    DEVICE_RESULTS = ("action_id", "traj_len", "traj_row", "traj_id", "status", "sc_flags", "path_len", "queue_cnt")
+
+    def device_results(self) -> dict:
+        """the last tick's results as torch views of the device buffers, without a copy or a synchronisation:
+        ``action_id``, ``traj_len``, ``traj_row``, ``traj_id``, ``status``, ``path_len`` [NSLOT][B], ``sc_flags`` [B],
+        ``queue_cnt`` (entry 2 = filled rows of ``traj``) and ``traj``, the compact export rows [(NSLOT + 1) * B]
+        [n_export][7] float32 (path (s, b) in row traj_row[s, b]).  For a caller that computes the next tick's
+        sel_action / pos_est on the device.  Work queued on the planner's stream after the tick sees them complete.
+        The views are valid until the next tick: it rewrites these buffers, and a stateful tick swaps planes by pointer,
+        so read or clone what is needed before staging the next tick."""
+        out = {n: self.t[n] for n in self.DEVICE_RESULTS}
+        out["traj"] = next(tb for tb in self.traj_bufs if tb.data_ptr() == self.buf.traj)
+        return out
 
     # -- result access (device -> host, test / facade use) ----------------------------------------------------------------------
     def fetch(self, *names) -> dict:

@@ -14,6 +14,7 @@ from __future__ import annotations
 from dataclasses import dataclass
 
 import numpy as np
+import torch
 
 from .lattice import import_globtraj_csv
 
@@ -94,6 +95,16 @@ class ScenarioBatch:
         """scenario i goes to rank i % world (SURVEY 8(e))."""
         return self.subset(np.arange(rank, self.size, world))
 
+    def to_device(self, device) -> "DeviceScenarioBatch":
+        """the same batch as torch tensors on `device` (DeviceScenarioBatch); DeviceScenarioBatch.cpu() gives it back
+        exactly"""
+        def dev(a, dt):
+            return None if a is None else torch.as_tensor(np.ascontiguousarray(a, dtype=dt)).to(device)
+        return DeviceScenarioBatch(dev(self.pos, np.float64), dev(self.heading, np.float64), dev(self.vel, np.float64),
+                                   dev(self.n_obj, np.int32), dev(self.obj, np.float64), self.zones,
+                                   dev(self.zone_sel, np.int32), dev(self.zone_key, np.int64),
+                                   dev(self.pred, np.float64), dev(self.n_pred, np.int32))
+
     @staticmethod
     def from_object_lists(pos, heading, vel, object_lists, k_max=None, blocked_zones=None) -> "ScenarioBatch":
         b = len(object_lists)
@@ -118,6 +129,88 @@ class ScenarioBatch:
         if blocked_zones is not None:
             sc.set_zones(blocked_zones)
         return sc
+
+
+@dataclass
+class DeviceScenarioBatch:
+    """A ScenarioBatch whose arrays already live on the device: torch tensors on the planner's device with the fields,
+    shapes and dtypes of ScenarioBatch.  Every tick entry point of BatchPlanner except plan_stream stages it with one
+    kernel (k_stage) instead of a host copy and an upload, and without a host synchronisation.  The tensors may be
+    non-contiguous: they are read through their strides, and ``obj`` may carry more than five columns, of which the
+    first five are used.  ``zones`` stays host data, as in ScenarioBatch; its bitmasks are uploaded when it changes."""
+    pos: torch.Tensor          # (B, 2)  float64
+    heading: torch.Tensor      # (B,)    float64
+    vel: torch.Tensor          # (B,)    float64
+    n_obj: torch.Tensor        # (B,)    int32
+    obj: torch.Tensor          # (B, K, >= 5) float64
+    zones: list = None
+    zone_sel: torch.Tensor = None   # (B,) int32
+    zone_key: torch.Tensor = None   # (B,) int64
+    pred: torch.Tensor = None       # (B, K, KP, 2) float64
+    n_pred: torch.Tensor = None     # (B, K) int32
+
+    _SPEC = (("pos", 2, torch.float64), ("heading", 1, torch.float64), ("vel", 1, torch.float64),
+             ("n_obj", 1, torch.int32), ("obj", 3, torch.float64), ("zone_sel", 1, torch.int32),
+             ("zone_key", 1, torch.int64), ("pred", 4, torch.float64), ("n_pred", 2, torch.int32))
+
+    @property
+    def size(self) -> int:
+        return int(self.pos.shape[0])
+
+    def subset(self, idx) -> "DeviceScenarioBatch":
+        """scenarios idx (a device index tensor, or anything torch indexing takes), as new tensors"""
+        def take(a):
+            return None if a is None else a[idx]
+        return DeviceScenarioBatch(take(self.pos), take(self.heading), take(self.vel), take(self.n_obj),
+                                   take(self.obj), self.zones, take(self.zone_sel), take(self.zone_key),
+                                   take(self.pred), take(self.n_pred))
+
+    def cpu(self) -> ScenarioBatch:
+        """the host ScenarioBatch of the same values (obj: its first five columns)"""
+        def host(a):
+            return None if a is None else a.cpu().numpy().copy()
+        return ScenarioBatch(host(self.pos), host(self.heading), host(self.vel), host(self.n_obj),
+                             host(self.obj[:, :, :5]), self.zones, host(self.zone_sel), host(self.zone_key),
+                             host(self.pred), host(self.n_pred))
+
+    def check(self, device) -> None:
+        """device, dtype, dimensionality and batch size of every tensor (ValueError); reads shapes only, no values"""
+        dev = torch.device(device)
+        for name, ndim, dt in self._SPEC:
+            a = getattr(self, name)
+            if a is None:
+                if name in ("pos", "heading", "vel", "n_obj", "obj"):
+                    raise ValueError("DeviceScenarioBatch.%s is required" % name)
+                continue
+            if not isinstance(a, torch.Tensor):
+                raise ValueError("DeviceScenarioBatch.%s must be a torch tensor, got %s" % (name, type(a).__name__))
+            if a.device.type != dev.type or (dev.index is not None and a.device.index != dev.index):
+                raise ValueError("DeviceScenarioBatch.%s is on %s, the planner on %s" % (name, a.device, dev))
+            if a.dtype != dt:
+                raise ValueError("DeviceScenarioBatch.%s must be %s, got %s" % (name, dt, a.dtype))
+            if a.dim() != ndim:
+                raise ValueError("DeviceScenarioBatch.%s must have %d dimensions, got shape %s" % (name, ndim,
+                                                                                                   tuple(a.shape)))
+        B, K = self.size, int(self.obj.shape[1])
+        if B < 1:
+            raise ValueError("DeviceScenarioBatch: the batch is empty")
+        want = dict(pos=(B, 2), obj=(B, K), n_pred=(B, K))
+        if self.pred is not None:
+            want["pred"] = (B, K, int(self.pred.shape[2]), 2)
+        for name, ndim, _ in self._SPEC:
+            a = getattr(self, name)
+            if a is None:
+                continue
+            shape = tuple(a.shape)
+            w = want.get(name, (B,))
+            if shape[:len(w)] != w:
+                raise ValueError("DeviceScenarioBatch.%s has shape %s, expected %s" % (name, shape, w + ("...",) *
+                                                                                       (ndim - len(w))))
+        if int(self.obj.shape[2]) < 5:
+            raise ValueError("DeviceScenarioBatch.obj needs at least 5 columns (X, Y, theta, v, length), got %d"
+                             % int(self.obj.shape[2]))
+        if (self.pred is None) != (self.n_pred is None):
+            raise ValueError("DeviceScenarioBatch: pred and n_pred come together")
 
 
 class Track(object):

@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define LTPL_ABI_VERSION 18
+#define LTPL_ABI_VERSION 19
 
 /* action ids (OTH:14-17 ACTION_ID_MAP) */
 #define LTPL_ACT_NONE (-1)
@@ -332,9 +332,35 @@ typedef struct LtplVelBatch {
     double* ax;                /* [n_paths][n_points] (last column 0)                                                    */
 } LtplVelBatch;
 
+/* Scenario inputs that already live on the device (ltpl_stage_inputs_batch): DEVICE pointers and strides, in elements,  */
+/* of the caller's arrays, read through their strides, so column slices and wider rows need no copy.  Scalars have one   */
+/* stride, [B][..] arrays one per dimension.                                                                             */
+typedef struct LtplStageSrc {
+    const double* pos;       int64_t pos_s[2];       /* [B][2]                                                         */
+    const double* heading;   int64_t heading_s;      /* [B]                                                            */
+    const double* vel;       int64_t vel_s;          /* [B]                                                            */
+    const double* vel_est;   int64_t vel_est_s;      /* [B]; NULL: vel                                                 */
+    const int32_t* n_obj;    int64_t n_obj_s;        /* [B]                                                            */
+    const double* obj;       int64_t obj_s[3];       /* [B][k_src][>= 5]: the first five columns (X, Y, theta, v, length) */
+    const double* pred;      int64_t pred_s[4];      /* [B][k_src][kp_src][2]; NULL: no object carries a prediction     */
+    const int32_t* n_pred;   int64_t n_pred_s[2];    /* [B][k_src]; with pred                                          */
+    const int32_t* zone_sel; int64_t zone_sel_s;     /* [B]; NULL: no zone (-1)                                        */
+    const int64_t* zone_key; int64_t zone_key_s;     /* [B] zone id key (0: none); NULL: all 0                         */
+    int64_t* zone_key_last;  /* [B] contiguous, read and written: the key of the previous staging; NULL: not kept      */
+    const void* sel_action;  int64_t sel_action_s;   /* [B] int32 or int64 (sel_action_bytes); NULL: not a stateful tick */
+    const double* t_const;   int64_t t_const_s;      /* [B]; NULL: t_const_value for every scenario                    */
+    const void* restart;     int64_t restart_s;      /* [B] 1-, 4- or 8-byte integers (restart_bytes), non-zero = restart */
+    double t_const_value;
+    int32_t k_src;           /* object slots of obj / n_pred / pred, <= dims.k_obj (the slots behind are zero-filled)     */
+    int32_t kp_src;          /* prediction points of pred, <= kp_dst                                                   */
+    int32_t kp_dst;          /* prediction points per slot of buffers.obj_pred (0: no obj_pred buffer)                 */
+    int32_t sel_action_bytes, restart_bytes;
+    int32_t zone_key_rule;   /* non-zero: a stateful tick, zone_s0[b] = -1 where the key changed and is non-zero        */
+} LtplStageSrc;
+
 int ltpl_version(void);
 const char* ltpl_last_error(void);
-int ltpl_sizeof(int which); /* 0 header, 1 params, 2 dims, 3 buffers, 4 velbatch: ABI self check for the ctypes mirror */
+int ltpl_sizeof(int which); /* 0 header, 1 params, 2 dims, 3 buffers, 4 velbatch, 5 stage src: ABI self check for the ctypes mirror */
 
 /* lattice handle over a caller-owned device blob -- replaces unpickling GraphBase (main_offline_callback.py:60-66)      */
 /* Fills the blob's follow table (search on the unblocked lattice from every node: one kernel on the legacy default  */
@@ -377,6 +403,13 @@ int ltpl_launch_stage(int stage, const LtplLattice* lat, const LtplParams* prm, 
                       const LtplBuffers* buf, void* stream);
 /* tph.calc_vel_profile(closed=False, loc_gg mode) over dense arrays                                                     */
 int ltpl_velprofile_batch(const LtplParams* prm, const LtplVelBatch* vb, void* stream);
+/* scenario inputs from device arrays, in ONE launch on the stream (k_stage): writes the input buffers of `buf` (pos,     */
+/* heading, vel, vel_est, n_obj, obj, zone_sel, n_pred, obj_pred; their const marks what the tick kernels do) with the   */
+/* bytes a host copy of the same arrays writes: obj slots k >= k_src and obj_pred behind the given points zero, n_pred   */
+/* -1 where no prediction is given, zone_sel -1 without zones.  With src.sel_action also sel_action and t_const, with     */
+/* src.restart buf.restart (0 / 1), with src.zone_key_rule the zone rule of a stateful tick (buf.zone_s0).  Values are     */
+/* taken as they are; the tick clamps n_obj, n_pred and zone_sel as it does for host inputs.                             */
+int ltpl_stage_inputs_batch(const LtplDims* dims, const LtplBuffers* buf, const LtplStageSrc* src, void* stream);
 
 /* number of kernel launches issued by this library since load (bench.py "gpu_launches")                                 */
 uint64_t ltpl_launch_count(void);

@@ -65,6 +65,24 @@ sel = pm.t["action_id"].max(dim=0).values.clamp(min=0).cpu().numpy()
 pm.next_tick(sc, sel_action=sel, t_const=0.1)
 r = pm.records()
 print("friction map stateful tick, trajectories:", sum(len(x.get("traj", {})) for x in r))
-mb =make_velocity_microbench(200, 150, seed=3)
+# scenario inputs from device tensors (k_stage): a first tick with predictions and zones from a DeviceScenarioBatch, then
+# a stateful tick with strided object columns, device sel_action / t_const / vel_est and a restart mask
+import torch
+sc = with_predictions(make_scenarios(Track(H.TRACK_CSV), n, seed=83, n_obj_min=0, n_obj_max=3), 6)
+sc.set_zones([{"z%d" % (b % 3): [[20 + b % 3, 20 + b % 3, 21], [0, 1, 0], None, None]} if b % 2 == 0 else None
+              for b in range(n)])
+pd = BatchPlanner(H.lattice_for("default"), device="cuda:0", stateful=True)
+pd.set_vel_params(ax_max_machines=g["ax_max_machines"], incl_emerg_traj=True, **VEL)
+dsc = sc.to_device("cuda:0")
+pd.stage_scenarios(dsc); pd.upload(); pd.set_startpos(); pd.tick()
+wide = torch.zeros((n, dsc.obj.shape[1], 8), dtype=torch.float64, device="cuda:0")
+wide[:, :, 2:7] = dsc.obj
+dsc.obj = wide[:, :, 2:]
+sel = pd.device_results()["action_id"].max(dim=0).values.clamp(min=0)
+pd.next_tick(dsc, sel, torch.full((n,), 0.1, dtype=torch.float64, device="cuda:0"), vel_est=dsc.vel * 0.9,
+             restart=torch.arange(n, device="cuda:0") % 5 == 0)
+r = pd.records()
+print("device inputs stateful tick, trajectories:", sum(len(x.get("traj", {})) for x in r))
+mb = make_velocity_microbench(200, 150, seed=3)
 vx, ax = calc_vel_profile_batch(pl, mb["kappa"], mb["el"], mb["v_start"], mb["v_end"])
 print("dense vx mean", float(np.mean(vx)))
