@@ -12,7 +12,7 @@ import os
 import subprocess
 import sys
 
-ABI_VERSION = 19
+ABI_VERSION = 20
 MAX_SUB = 8
 NSLOT = 3
 MAX_AXM = 32
@@ -82,7 +82,7 @@ BUFFER_FIELDS = ("pos", "heading", "vel", "vel_est", "n_obj", "obj", "sc_flags",
                  "n_pred", "prev_path", "prev_path_len", "prev_node_idx", "prev_nodes", "prev_n_nodes", "prev_coeff",
                  "prev_s_vx_ax", "prev_action_id", "prev_traj_len", "prev_trim", "sel_action", "pos_last", "t_const",
                  "st_info", "trim", "vel_plan", "course", "obj_dist", "zone_s0", "em_vx", "prev_em_vx", "prev_em_info",
-                 "gg", "prev_gg", "restart", "gg_map")
+                 "gg", "prev_gg", "restart", "gg_map", "traj_base")
 STATE_FIELDS = BUFFER_FIELDS[BUFFER_FIELDS.index("prev_path"):]   # NULL unless a stateful tick is planned
 
 
@@ -111,7 +111,7 @@ EXPORTS = ("ltpl_version", "ltpl_last_error", "ltpl_sizeof", "ltpl_max_objects",
            "ltpl_lattice_destroy", "ltpl_set_startpos_batch", "ltpl_calc_paths_batch", "ltpl_calc_vel_profile_batch",
            "ltpl_tick_batch", "ltpl_velprofile_batch", "ltpl_launch_count", "ltpl_launch_stage", "ltpl_next_tick_batch",
            "ltpl_next_calc_paths_batch", "ltpl_next_calc_vel_profile_batch", "ltpl_set_subbatches",
-           "ltpl_stage_inputs_batch")
+           "ltpl_stage_inputs_batch", "ltpl_prepare_batch")
 
 
 def build_library(verbose: bool = False) -> str:
@@ -169,6 +169,8 @@ def load_library():
     lib.ltpl_velprofile_batch.restype = C.c_int
     lib.ltpl_stage_inputs_batch.argtypes = [C.POINTER(Dims), C.POINTER(Buffers), C.POINTER(StageSrc), C.c_void_p]
     lib.ltpl_stage_inputs_batch.restype = C.c_int
+    lib.ltpl_prepare_batch.argtypes = [C.c_void_p, C.POINTER(Params), C.POINTER(Dims), C.POINTER(Buffers)]
+    lib.ltpl_prepare_batch.restype = C.c_int
     if lib.ltpl_version() != ABI_VERSION:
         raise RuntimeError("libltpl_b200.so ABI version %d != binding %d" % (lib.ltpl_version(), ABI_VERSION))
     for which, st in enumerate((LatticeHeader, Params, Dims, Buffers, VelBatch, StageSrc)):

@@ -22,6 +22,7 @@
 #include "ltpl_smooth.cuh"
 #include "ltpl_gg_map.cuh"
 #include "ltpl_stage.cuh"
+#include "ltpl_traj_base.cuh"
 
 // the memory records are the int32 arrays BatchPlanner allocates: st_info [B][8], trim [NSLOT*B][4]
 static_assert(sizeof(LtplStateInfo) == 8 * sizeof(int32_t) && alignof(LtplStateInfo) == alignof(int32_t), "st_info row");
@@ -108,13 +109,18 @@ static const PlanFn kPlanFns[8] = {k_plan<false, false, false>, k_plan<true, fal
                                    k_plan<true, true, false>,   k_plan<false, false, true>, k_plan<true, false, true>,
                                    k_plan<false, true, true>,   k_plan<true, true, true>};
 
-static int launch_k_plan(const LtplLattice* lat, const LtplParams* prm, const LtplDims* dm, const LtplBuffers* bf,
-                         cudaStream_t st, bool stateful) {
+static size_t plan_smem(const LtplLattice* lat, const LtplDims* dm) {
+    return plan_smem_bytes_per_warp(plan_maxn(&lat->h), dm->h_max, plan_mask_words(&lat->h), dm->k_obj) *
+           LTPL_WARPS_PER_CTA;
+}
+
+// k_plan's attributes for these dims: the dynamic shared-memory limit and the carveout (set when they change)
+static int plan_attributes(const LtplLattice* lat, const LtplDims* dm) {
     const int maxn = plan_maxn(&lat->h);
     const int hl = dm->h_max;
     const int mask_words = plan_mask_words(&lat->h);
-    const size_t smem = plan_smem_bytes_per_warp(maxn, hl, mask_words, dm->k_obj) * LTPL_WARPS_PER_CTA;
-    if (int r = allow_smem(lat, kSmemPlan, smem, kPlanFns, "k_plan", "lattice window too large for shared memory"))
+    if (int r = allow_smem(lat, kSmemPlan, plan_smem(lat, dm), kPlanFns, "k_plan",
+                           "lattice window too large for shared memory"))
         return r;
     // Shared-memory carveout: what LTPL_PLAN_MINB CTAs need with at least 16 object slots (1 KB reserved per CTA, 228 KB
     // per sm_90 SM).  For fewer slots the driver would pick a smaller carveout (more L1) for k_plan, and the benchmark
@@ -132,6 +138,16 @@ static int launch_k_plan(const LtplLattice* lat, const LtplParams* prm, const Lt
             }
         lat->plan_carveout = carveout;
     }
+    return 0;
+}
+
+static int launch_k_plan(const LtplLattice* lat, const LtplParams* prm, const LtplDims* dm, const LtplBuffers* bf,
+                         cudaStream_t st, bool stateful) {
+    if (int r = plan_attributes(lat, dm)) return r;
+    const int maxn = plan_maxn(&lat->h);
+    const int hl = dm->h_max;
+    const int mask_words = plan_mask_words(&lat->h);
+    const size_t smem = plan_smem(lat, dm);
     const bool zone = dm->n_zones > 0;
     const bool dense = lat->h.num_edges >= 2 * lat->h.num_nodes;   // in-edges per node (dp_run<.., DENSE>)
     kPlanFns[(zone ? 1 : 0) + (stateful ? 2 : 0) + (dense ? 4 : 0)]<<<ctas(dm->sub_cnt), kThreads, smem, st>>>(
@@ -140,36 +156,50 @@ static int launch_k_plan(const LtplLattice* lat, const LtplParams* prm, const Lt
 }
 
 // k_path<STATE>: one warp per path (ltpl_path.cuh)
+typedef void (*PathFn)(const __grid_constant__ LatDev, const __grid_constant__ LtplParams, const __grid_constant__ LtplDims,
+                       const __grid_constant__ LtplBuffers);
+static const PathFn kPathFns[2] = {k_path<false>, k_path<true>};
+
+static size_t path_smem(const LtplDims* dm) { return path_smem_bytes_per_warp(dm->h_max) * LTPL_WARPS_PER_CTA; }
+
+static int path_attributes(const LtplLattice* lat, const LtplDims* dm) {
+    return allow_smem(lat, kSmemPath, path_smem(dm), kPathFns, "k_path", "lattice window too large for shared memory");
+}
+
 static int launch_k_path(const LtplLattice* lat, const LtplParams* prm, const LtplDims* dm, const LtplBuffers* bf,
                          cudaStream_t st, bool stateful) {
-    const size_t smem = path_smem_bytes_per_warp(dm->h_max) * LTPL_WARPS_PER_CTA;
-    typedef void (*PathFn)(const __grid_constant__ LatDev, const __grid_constant__ LtplParams,
-                           const __grid_constant__ LtplDims, const __grid_constant__ LtplBuffers);
-    static const PathFn fns[2] = {k_path<false>, k_path<true>};
-    if (int r = allow_smem(lat, kSmemPath, smem, fns, "k_path", "lattice window too large for shared memory")) return r;
-    fns[stateful]<<<ctas(LTPL_NSLOT * dm->sub_cnt), kThreads, smem, st>>>(lat->d, *prm, *dm, *bf);
+    const size_t smem = path_smem(dm);
+    if (int r = path_attributes(lat, dm)) return r;
+    kPathFns[stateful]<<<ctas(LTPL_NSLOT * dm->sub_cnt), kThreads, smem, st>>>(lat->d, *prm, *dm, *bf);
     return check_launch("k_path");
 }
 
 // velocity kernel: one CTA per VR_P queued paths of one class, the paths resident in shared memory (ltpl_vel_res.cuh)
-static int launch_k_vel(const LtplLattice* lat, const LtplParams* prm, const LtplDims* dm, const LtplBuffers* bf,
-                        cudaStream_t st, bool stateful) {
+typedef void (*VelFn)(const LatDev, const LtplParams, const LtplDims, const LtplBuffers, const int);
+// <STATE, EXP1, GG>: [stateful + 2 * (0 exponent 1, 1 general exponent, 2 local_gg planes)]
+static const VelFn kVelFns[6] = {k_vel_res<false, true, false>, k_vel_res<true, true, false>,
+                                 k_vel_res<false, false, false>, k_vel_res<true, false, false>,
+                                 k_vel_res<false, false, true>, k_vel_res<true, false, true>};
+
+static int vel_attributes(const LtplLattice* lat, const LtplDims* dm, const LtplBuffers* bf) {
     const int nmax = dm->p_max;
     if (nmax > 32 * VR_MAXM)
         return fail("k_vel: dims.p_max exceeds the shared-memory capacity of the velocity kernel (<= 512)");
-    const bool gg = bf->gg != nullptr;   // location dependent local_gg: the general-exponent variant carries it
+    // location dependent local_gg: the general-exponent variant carries it
+    return allow_smem(lat, kSmemVel, vr_smem_bytes(nmax, bf->gg != nullptr), kVelFns, "k_vel",
+                      "dims.p_max too large for the velocity kernel's shared memory");
+}
+
+static int launch_k_vel(const LtplLattice* lat, const LtplParams* prm, const LtplDims* dm, const LtplBuffers* bf,
+                        cudaStream_t st, bool stateful) {
+    if (int r = vel_attributes(lat, dm, bf)) return r;
+    const int nmax = dm->p_max;
+    const bool gg = bf->gg != nullptr;
     const size_t smem = vr_smem_bytes(nmax, gg);
-    typedef void (*VelFn)(const LatDev, const LtplParams, const LtplDims, const LtplBuffers, const int);
-    // <STATE, EXP1, GG>: [stateful + 2 * (0 exponent 1, 1 general exponent, 2 local_gg planes)]
-    static const VelFn fns[6] = {k_vel_res<false, true, false>, k_vel_res<true, true, false>,
-                                 k_vel_res<false, false, false>, k_vel_res<true, false, false>,
-                                 k_vel_res<false, false, true>, k_vel_res<true, false, true>};
-    if (int r = allow_smem(lat, kSmemVel, smem, fns, "k_vel", "dims.p_max too large for the velocity kernel's shared memory"))
-        return r;
     const int kind = gg ? 2 : (prm->dyn_model_exp == 1.0 ? 0 : 1);
     const int nq = LTPL_NSLOT * dm->sub_cnt;   // paths of this launch's scenario window
     const int grid = nq / VR_P + 2;            // >= groups of the follow queue + groups of the other queue
-    fns[(stateful ? 1 : 0) + 2 * kind]<<<grid, VR_THREADS, smem, st>>>(lat->d, *prm, *dm, *bf, nmax);
+    kVelFns[(stateful ? 1 : 0) + 2 * kind]<<<grid, VR_THREADS, smem, st>>>(lat->d, *prm, *dm, *bf, nmax);
     return check_launch("k_vel");
 }
 
@@ -423,6 +453,11 @@ static int validate(const LtplLattice* lat, const LtplParams* prm, const LtplDim
         if (!std::isfinite(prm->gg_map_x0) || !std::isfinite(prm->gg_map_y0))
             return fail("params.gg_map_x0 and params.gg_map_y0 must be finite");
     }
+    if (bf->traj_base) {   // ids from the device counter (k_traj_base)
+        if (prm->traj_base_id != 0)
+            return fail("buffers.traj_base needs params.traj_base_id = 0: k_traj_base adds the base from the counter");
+        if (reinterpret_cast<uintptr_t>(bf->traj_base) % 4 != 0) return fail("buffers.traj_base must be 4-byte aligned");
+    }
     if (!stateful) return 0;
     if (!bf->prev_path || !bf->prev_path_len || !bf->prev_node_idx || !bf->prev_nodes || !bf->prev_n_nodes ||
         !bf->prev_coeff || !bf->prev_s_vx_ax || !bf->prev_action_id || !bf->prev_traj_len || !bf->prev_trim ||
@@ -541,11 +576,17 @@ static int run_tick(const LtplLattice* lat, const LtplParams* prm, const LtplDim
     // planned velocity at the cut instead
     LtplBuffers vbf = *bf;
     if (stateful) vbf.vel = bf->vel_plan;
-    return for_windows(lat, dm, st, [&](const LtplDims* w, cudaStream_t s) {
-        if (paths)
-            if (int r = paths_window(lat, prm, w, bf, s, stateful)) return r;
-        return vel ? vel_window(lat, prm, w, &vbf, s, stateful) : 0;
-    });
+    if (int r = for_windows(lat, dm, st, [&](const LtplDims* w, cudaStream_t s) {
+            if (paths)
+                if (int r = paths_window(lat, prm, w, bf, s, stateful)) return r;
+            return vel ? vel_window(lat, prm, w, &vbf, s, stateful) : 0;
+        }))
+        return r;
+    if (!vel || !bf->traj_base) return 0;
+    // trajectory ids from the device counter, behind the join: every window's ids are written
+    k_traj_base<<<1, LTPL_TRAJ_BASE_THREADS, 0, st>>>(bf->traj_base, bf->traj_id, prm->incl_emerg_traj ? bf->em_info : nullptr,
+                                                      (int)(LTPL_NSLOT * B), (int)B);
+    return check_launch("k_traj_base");
 }
 
 int ltpl_calc_paths_batch(const LtplLattice* lat, const LtplParams* prm, const LtplDims* dm, const LtplBuffers* bf,
@@ -579,6 +620,13 @@ int ltpl_next_calc_vel_profile_batch(const LtplLattice* lat, const LtplParams* p
 int ltpl_next_tick_batch(const LtplLattice* lat, const LtplParams* prm, const LtplDims* dm, const LtplBuffers* bf,
                          void* stream) {
     return run_tick(lat, prm, dm, bf, stream, kPaths | kVel, true);
+}
+
+int ltpl_prepare_batch(const LtplLattice* lat, const LtplParams* prm, const LtplDims* dm, const LtplBuffers* bf) {
+    if (int r = validate(lat, prm, dm, bf, false)) return r;
+    if (int r = plan_attributes(lat, dm)) return r;
+    if (int r = path_attributes(lat, dm)) return r;
+    return vel_attributes(lat, dm, bf);
 }
 
 int ltpl_launch_stage(int stage, const LtplLattice* lat, const LtplParams* prm, const LtplDims* dm,

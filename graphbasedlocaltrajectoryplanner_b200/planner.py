@@ -157,6 +157,9 @@ class BatchPlanner(object):
         self._staged_on_device = False   # the last staged batch was a DeviceScenarioBatch: upload() has nothing to copy
         self._zones_dev = None        # the zone list whose bitmasks the device path uploaded last (None: none / stale)
         self._zone_key_dev = None     # [B] int64: zone keys of the last device staging (k_stage reads and writes it)
+        self._generation = 0          # bumped by every change a captured TickGraph cannot follow (tick_graph.py)
+        self._ticked = False          # the buffers hold a tick (a velocity call ran since they were allocated)
+        self._traj_base = None        # [1] int32 device id counter of buffers.traj_base, from the first capture on
         self.set_vel_params()
 
     def __del__(self):
@@ -172,6 +175,7 @@ class BatchPlanner(object):
         of >= 512 scenarios): window s runs on an internal stream, so kernels of different stages overlap.  The results
         do not depend on it (only the unspecified order of the compact export rows)."""
         capi.check(self.lib, self.lib.ltpl_set_subbatches(self.handle, int(n)), "ltpl_set_subbatches")
+        self._generation += 1
 
     # -- parameters ------------------------------------------------------------------------------------------------------
     def set_vel_params(self, vel_max: float = 100.0, gg_scale: float = 1.0, local_gg=(5.0, 5.0),
@@ -189,6 +193,7 @@ class BatchPlanner(object):
             raise ValueError("ax_max_machines has more than %d rows" % capi.MAX_AXM)
         if axm[-1, 0] < vel_max:                               # tph.calc_vel_profile input check
             raise RuntimeError("ax_max_machines has to cover the entire velocity range of the car (i.e. >= v_max)!")
+        self._generation += 1   # after the checks: a refused call leaves captured graphs valid
         p = self.params
         o = self.online
         p.max_heading_offset = o["max_heading_offset"]
@@ -276,6 +281,7 @@ class BatchPlanner(object):
             # more object slots / prediction points than before: only the input buffers grow (see _alloc_inputs)
             torch.cuda.current_stream(self.device).synchronize()
             self._alloc_inputs(batch, max(k_obj, self.dims.k_obj), max(int(k_pred), self._k_pred_cap))
+            self._generation += 1
             return
         d = capi.Dims()
         d.batch, d.k_obj = int(batch), k_obj
@@ -311,6 +317,10 @@ class BatchPlanner(object):
             if name not in capi.STATE_FIELDS and name in t:   # `trim` is a state field: NULL unless the planner is stateful
                 setattr(buf, name, t[name].data_ptr())
         self.t, self.buf, self.dims = t, buf, d
+        self._generation += 1
+        self._ticked = False
+        if self._traj_base is not None:
+            buf.traj_base = self._traj_base.data_ptr()
         self._gg_planes_used = False
         self._zones_dev = None
         self._alloc_inputs(B, k_obj, k_pred)
@@ -338,9 +348,12 @@ class BatchPlanner(object):
         straight | follow, 1: left, 2: right), aligned with the paths of the last calc_paths; None: back to the constant
         tuple of set_vel_params().  The values are taken without gg_scale (VPFB:213-214 applies it).  Clears the friction
         map of set_gg_map()."""
+        if self._gg_map is not None:   # captured graphs evaluate the map: they go stale with it
+            self._generation += 1
         self._gg_map = None
         self.buf.gg_map = None
         if ax is None:
+            self._generation += 1
             self.buf.gg = None
             return
         ax = np.asarray(ax, dtype=np.float64)
@@ -348,6 +361,7 @@ class BatchPlanner(object):
         B, P = self.dims.batch, self.dims.p_max
         if ax.shape != ay.shape or ax.ndim != 3 or ax.shape[:2] != (NSLOT, B) or ax.shape[2] > P:
             raise ValueError("local_gg planes must have the shape [NSLOT][B][P <= p_max]")
+        self._generation += 1
         if "gg" not in self.t:
             self.t["gg"] = torch.ones((2, NSLOT * B, P), dtype=torch.float64, device=self.device)
         host = np.ones((2, NSLOT * B, P))
@@ -366,6 +380,7 @@ class BatchPlanner(object):
         and stays until it is changed.  None: back to the constant tuple of set_vel_params().  Clears the planes of
         set_local_gg_planes().  Bad input raises ValueError and changes nothing."""
         if ax is None:
+            self._generation += 1
             self._gg_map = None
             if self.buf is not None:
                 self.buf.gg_map = None
@@ -385,6 +400,7 @@ class BatchPlanner(object):
         p = self.params
         p.gg_map_x0, p.gg_map_y0, p.gg_map_inv_cell = float(x0), float(y0), inv_cell
         p.gg_map_nx, p.gg_map_ny = nx, ny
+        self._generation += 1
         self._bind_gg_map()
 
     def _bind_gg_map(self) -> None:
@@ -544,20 +560,26 @@ class BatchPlanner(object):
         if restart is not None:
             put("restart", restart)
             src.restart_bytes = restart.element_size()
-        # the zone key of the last staging lives on the device from now on; after a host staging it crosses over once
+        kept = self._cross_zone_key()
+        src.zone_key_rule = int(zone_rule and kept)
+        src.zone_key_last = self._zone_key_dev.data_ptr()
+        self._stage_zones_device(sc.zones)
+        self._staged_on_device = True
+        capi.check(self.lib, self.lib.ltpl_stage_inputs_batch(C.byref(self.dims), C.byref(self.buf), C.byref(src),
+                                                              self.stream), "ltpl_stage_inputs_batch")
+
+    def _cross_zone_key(self) -> bool:
+        """the zone key of the last staging lives on the device from now on (_zone_key_dev, which k_stage reads and
+        writes); after a host staging it crosses over once.  Returns whether the last staging kept a key of this batch
+        size (the zone key rule of a stateful tick applies)."""
         B = self.dims.batch
         last = getattr(self, "_zone_key", None)
         if self._zone_key_dev is None or self._zone_key_dev.shape[0] != B:
             self._zone_key_dev = torch.zeros((B,), dtype=torch.int64, device=self.device)
         if isinstance(last, np.ndarray) and last.shape == (B,):
             self._zone_key_dev.copy_(torch.from_numpy(last))
-        src.zone_key_last = self._zone_key_dev.data_ptr()
-        src.zone_key_rule = int(zone_rule and last is not None and tuple(last.shape) == (B,))
         self._zone_key = self._zone_key_dev
-        self._stage_zones_device(sc.zones)
-        self._staged_on_device = True
-        capi.check(self.lib, self.lib.ltpl_stage_inputs_batch(C.byref(self.dims), C.byref(self.buf), C.byref(src),
-                                                              self.stream), "ltpl_stage_inputs_batch")
+        return last is not None and tuple(last.shape) == (B,)
 
     def _stage_zones_device(self, zones) -> None:
         """zone bitmasks of a device batch: uploaded (pinned, asynchronously) only when the zone list changed"""
@@ -710,11 +732,14 @@ class BatchPlanner(object):
                                                      C.byref(self.buf), self.stream), name)
 
     def _call_vel(self, name):
-        """a call that includes calc_vel_profile: its trajectories get the next ids (+10 per call, OTH:669)"""
+        """a call that includes calc_vel_profile: its trajectories get the next ids (+10 per call, OTH:669).  Once a
+        TickGraph was captured on this planner the ids come from the device counter buffers.traj_base (k_traj_base),
+        so that eager calls and replays number alike."""
         self._tick_count += 1
-        self.params.traj_base_id = 10 * self._tick_count
+        self.params.traj_base_id = 10 * self._tick_count if self._traj_base is None else 0
         self._call(name)
         self._gg_planes_used = self.buf.gg is not None
+        self._ticked = True
 
     def set_startpos(self) -> None:
         self._call("ltpl_set_startpos_batch")
@@ -897,6 +922,85 @@ class BatchPlanner(object):
         poses of the scenarios ``restart`` marks, see next_calc_paths)."""
         self._stage_next(sc, sel_action, t_const, vel_est, restart)   # vel_est travels in the packed upload
         self._call_vel("ltpl_next_tick_batch")
+
+    # -- ticks replayed from CUDA graphs (tick_graph.py, DESIGN.md section 11) -------------------------------------------
+    def capture_tick(self, sc, vel_est=None, restart=None):
+        """capture a first tick -- k_stage + set_startpos + tick of ``sc`` (a DeviceScenarioBatch) -- into a CUDA graph
+        and return a TickGraph: write each tick's inputs into ``graph.inputs`` (TickInputs.copy_) and call
+        ``graph.replay()``, which enqueues the tick with no host work.  The arguments are those of the eager device
+        calls.  Everything that could allocate or copy from the host happens here, before the capture (a batch of
+        another size starts a new session, as in stage_scenarios); the zone list ``sc.zones`` is fixed for the graph's
+        lifetime.  Nothing is launched and the planner's state is left as it was."""
+        from .tick_graph import capture
+        if restart is not None:
+            raise ValueError("capture_tick: a first tick takes no restart mask (capture_next_tick does)")
+        return capture(self, False, sc, vel_est=vel_est)
+
+    def capture_next_tick(self, sc, sel_action, t_const, vel_est=None, restart=None):
+        """capture a stateful tick (next_tick with the same arguments) into CUDA graphs, one per ping-pong parity of
+        the planner's buffers, and return a TickGraph (see capture_tick).  A replay runs the graph of the planner's
+        current parity and then does the host side of the tick (pointer swaps, tick count), so eager ticks and replays
+        may be interleaved freely.  Needs a previous tick in this session and the session's batch size."""
+        from .tick_graph import capture
+        return capture(self, True, sc, vel_est=vel_est, sel_action=sel_action, t_const=t_const, restart=restart)
+
+    def _prepare_capture(self, inputs, stateful: bool) -> None:
+        """everything a tick of these inputs could allocate, grow or copy from the host, done before a capture: the
+        buffers for the batch, the memory buffers a stateful tick creates on first use, the zone key crossing over from
+        a host staging, the zone bitmasks, the id counter and the kernels' attributes (ltpl_prepare_batch)"""
+        sc = inputs.sc
+        pos = self.t["pos"] if stateful else None
+        self._grow_for(sc)
+        if pos is not None and self.t["pos"] is not pos:
+            # more object slots or prediction points: the input copies were re-created (the current one is copy 0).  A
+            # stateful tick reads the last tick's positions as pos_last from the current copy; the eager tick keeps the
+            # old copy for it instead, so the current copy takes its values here
+            self.t["pos"].copy_(pos)
+        if stateful:
+            if self._state is None:
+                self._alloc_state()
+            if inputs.restart is not None:
+                self._restart_buffer()
+            if "gg" in self.t and "gg" not in self._state["other"]:   # what the first gg swap would create
+                self._state["other"]["gg"] = torch.ones_like(self.t["gg"])
+        if getattr(self, "_zone_key", None) is not None:
+            self._cross_zone_key()
+        elif self._zone_key_dev is None or self._zone_key_dev.shape[0] != self.dims.batch:
+            self._zone_key_dev = torch.zeros((self.dims.batch,), dtype=torch.int64, device=self.device)
+        self._stage_zones_device(sc.zones)
+        if self._traj_base is None:   # the ids an all-eager session would give next
+            self._traj_base = torch.full((1,), 10 * self._tick_count, dtype=torch.int32, device=self.device)
+        self.buf.traj_base = self._traj_base.data_ptr()
+        self.params.traj_base_id = 0
+        capi.check(self.lib, self.lib.ltpl_prepare_batch(self.handle, C.byref(self.params), C.byref(self.dims),
+                                                         C.byref(self.buf)), "ltpl_prepare_batch")
+
+    _TICK_ATTRS = ("_in_cur", "d_in_raw", "_pos_last", "_gg_planes_used", "_zone_key", "_zones_dev",
+                   "_staged_on_device", "_ticked")
+
+    def _host_state(self) -> dict:
+        """what a tick changes on the host: the pointer fields and dims a call passes, the buffer dicts (by reference)
+        and the host mirrors"""
+        return dict(buf=capi.Buffers.from_buffer_copy(self.buf), dims=capi.Dims.from_buffer_copy(self.dims),
+                    t=dict(self.t), other=None if self._state is None else dict(self._state["other"]),
+                    attrs={k: getattr(self, k, None) for k in self._TICK_ATTRS})
+
+    def _set_host_state(self, hs: dict) -> None:
+        C.memmove(C.addressof(self.buf), C.addressof(hs["buf"]), C.sizeof(capi.Buffers))
+        C.memmove(C.addressof(self.dims), C.addressof(hs["dims"]), C.sizeof(capi.Dims))
+        self.t.clear()
+        self.t.update(hs["t"])
+        if hs["other"] is not None:
+            self._state["other"].clear()
+            self._state["other"].update(hs["other"])
+        for k, v in hs["attrs"].items():
+            setattr(self, k, v)
+
+    def _tick_key(self, stateful: bool) -> tuple:
+        """the buffers the next tick would use: the input copy, the ping-pong planes, the gg planes and, for a stateful
+        tick, whether the last velocity call ran with planes (it decides the gg swap and prev_gg)"""
+        key = (self._in_cur,) + tuple(self.t[k].data_ptr() if k in self.t else 0 for k in self._BIG + ("gg",))
+        return key + (self._gg_planes_used,) if stateful else key
 
     def launch_count(self) -> int:
         return int(self.lib.ltpl_launch_count())

@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define LTPL_ABI_VERSION 19
+#define LTPL_ABI_VERSION 20
 
 /* action ids (OTH:14-17 ACTION_ID_MAP) */
 #define LTPL_ACT_NONE (-1)
@@ -318,6 +318,14 @@ typedef struct LtplBuffers {
     /* bilinear interpolation at every path point (k_gg_map, DESIGN.md section 7) -- calc_vel_profile(local_gg={action:    */
     /* [map(path[:, 0:2])]}).  Needs `gg` and 16-byte alignment.  NULL: `gg` is read as the caller left it.               */
     const double* gg_map;           /* [ny][nx][2] ax_max, ay_max per vertex (without gg_scale), one 16-byte pair each     */
+    /* trajectory ids from a device counter, for ticks replayed from a CUDA graph (the id base of params.traj_base_id     */
+    /* would be frozen at capture): the velocity stage of every entry point then ends with k_traj_base on the caller's    */
+    /* stream, which advances *traj_base by 10 and adds the new value to the ids this call wrote -- every traj_id in     */
+    /* [0, 10) and, with params.incl_emerg_traj, every emergency id in [0, 10) (em_info[b][2] where em_info[b][0] >= 0)  */
+    /* -- giving the bytes of the same call with params.traj_base_id = the new value.  Ids of earlier calls are >= 10    */
+    /* and stay as they are.  Needs params.traj_base_id = 0, a counter >= 0 and 4-byte alignment.  NULL: the ids are      */
+    /* params.traj_base_id + action id, and nothing extra is launched.                                                    */
+    int32_t* traj_base;             /* [1] the id base of the last velocity stage (an all-eager session: 10 * its calls)  */
 } LtplBuffers;
 
 /* stand-alone forward/backward ggv velocity profile over dense path arrays (BASELINE.json config 5).                   */
@@ -410,6 +418,12 @@ int ltpl_velprofile_batch(const LtplParams* prm, const LtplVelBatch* vb, void* s
 /* src.restart buf.restart (0 / 1), with src.zone_key_rule the zone rule of a stateful tick (buf.zone_s0).  Values are     */
 /* taken as they are; the tick clamps n_obj, n_pred and zone_sel as it does for host inputs.                             */
 int ltpl_stage_inputs_batch(const LtplDims* dims, const LtplBuffers* buf, const LtplStageSrc* src, void* stream);
+
+/* Sets, for these lattice / params / dims / buffers, every per-kernel attribute a tick entry point would otherwise set   */
+/* on its first launch (dynamic shared-memory limits of k_plan, k_path and the velocity kernel, k_plan's carveout);      */
+/* launches nothing.  Call it before capturing a tick into a CUDA graph: attribute calls are not allowed while a stream */
+/* is being captured.  The velocity kernel's limit depends on buf->gg (planes or the constant tuple).                   */
+int ltpl_prepare_batch(const LtplLattice* lat, const LtplParams* prm, const LtplDims* dims, const LtplBuffers* buf);
 
 /* number of kernel launches issued by this library since load (bench.py "gpu_launches")                                 */
 uint64_t ltpl_launch_count(void);

@@ -83,6 +83,15 @@ pd.next_tick(dsc, sel, torch.full((n,), 0.1, dtype=torch.float64, device="cuda:0
              restart=torch.arange(n, device="cuda:0") % 5 == 0)
 r = pd.records()
 print("device inputs stateful tick, trajectories:", sum(len(x.get("traj", {})) for x in r))
+# a stateful tick captured into CUDA graphs (one per ping-pong parity, k_traj_base behind the windows) and replayed 4
+# times with the next sel_action copied into its inputs
+graph = pd.capture_next_tick(dsc, sel, 0.1, vel_est=dsc.vel * 0.9)
+for _ in range(4):
+    graph.inputs.copy_(dsc, pd.device_results()["action_id"].max(dim=0).values.clamp(min=0), vel_est=dsc.vel * 0.9)
+    graph.replay()
+graph.close()
+r = pd.records()
+print("replayed stateful tick, trajectories:", sum(len(x.get("traj", {})) for x in r))
 mb = make_velocity_microbench(200, 150, seed=3)
 vx, ax = calc_vel_profile_batch(pl, mb["kappa"], mb["el"], mb["v_start"], mb["v_end"])
 print("dense vx mean", float(np.mean(vx)))
