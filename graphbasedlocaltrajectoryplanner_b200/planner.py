@@ -14,6 +14,7 @@ from __future__ import annotations
 import configparser
 import ctypes as C
 import json
+from dataclasses import dataclass, replace
 
 import numpy as np
 import torch
@@ -102,6 +103,20 @@ DEFAULT_ONLINE = dict(max_heading_offset=0.8, nmbr_export_points=115, v_max_offs
                       control_params={"c_p": 1.25, "k_d": 0.025, "k_p": 0.2}, delaycomp=0.1)
 
 
+@dataclass
+class TickState:
+    """what a tick changes on the planner's host side besides the pointer fields (buffers), dims and the buffer dicts.
+    A TickGraph keeps a copy of it per captured state and installs that copy after a replay."""
+    in_cur: int = 0                  # the device input copy in use (stateful ticks alternate the two)
+    pos_last: torch.Tensor = None    # `pos` of the input copy the last tick used: buffers.pos_last of a stateful tick
+    gg_planes_used: bool = False     # the last velocity call ran with gg planes (decides the next tick's prev_gg)
+    zone_key_kept: bool = False      # a staging since allocate(): the next stateful tick applies the zone rule
+    zone_key_zero: bool = True       # the device zone keys (_zone_key) are all zero
+    zones: tuple = None              # the zone list whose bitmasks are on the device (None: none yet)
+    staged_on_device: bool = False   # the last staged batch was a DeviceScenarioBatch: upload() has nothing to copy
+    ticked: bool = False             # the buffers hold a tick (a velocity call ran since they were allocated)
+
+
 class BatchPlanner(object):
     N_SETS = 3   # host staging / export buffer sets of the pipelined path (plan_stream)
 
@@ -110,6 +125,7 @@ class BatchPlanner(object):
                  blob_tensor: torch.Tensor = None, stateful: bool = False):
         """``packed`` = (LatticeHeader, capacities) + ``blob_tensor`` (device uint8) when the blob arrived through a
         collective instead of being uploaded from ``lattice`` (parallel.broadcast_lattice)."""
+        self.handle = None
         self.online = dict(DEFAULT_ONLINE)
         if online:
             self.online.update(online)
@@ -150,21 +166,16 @@ class BatchPlanner(object):
         self.params = capi.Params()
         self._tick_count = 0
         self._gg_map = None           # device [ny][nx][2] friction map of set_gg_map, or None
-        # whether the velocity half of the last tick ran with gg planes (uploaded or from the map): decides whether the
-        # next stateful tick brakes on its backup plan with those planes (prev_gg) or with the constant tuple
-        self._gg_planes_used = False
         self.on_device_start = None   # optional callable, called where a stateful tick's host staging ends (timing)
-        self._staged_on_device = False   # the last staged batch was a DeviceScenarioBatch: upload() has nothing to copy
-        self._zones_dev = None        # the zone list whose bitmasks the device path uploaded last (None: none / stale)
-        self._zone_key_dev = None     # [B] int64: zone keys of the last device staging (k_stage reads and writes it)
+        self._tick = TickState()
         self._generation = 0          # bumped by every change a captured TickGraph cannot follow (tick_graph.py)
-        self._ticked = False          # the buffers hold a tick (a velocity call ran since they were allocated)
         self._traj_base = None        # [1] int32 device id counter of buffers.traj_base, from the first capture on
+        self._copy_stream = None      # second stream of plan_stream (trajectory downloads), created on first use
         self.set_vel_params()
 
     def __del__(self):
         try:
-            if getattr(self, "handle", None):
+            if self.handle:
                 self.lib.ltpl_lattice_destroy(self.handle)
                 self.handle = None
         except Exception:
@@ -266,12 +277,21 @@ class BatchPlanner(object):
         self._use_inputs(0)
 
     def _use_inputs(self, which: int) -> None:
-        self._in_cur = which
-        self.d_in_raw, views = self.d_in[which]
+        self._tick.in_cur = which
+        views = self.d_in[which][1]
         self.t.update(views)
         for name in self._IN_NAMES:
             if name in views and name not in ("sel_action", "t_const"):
                 setattr(self.buf, name, views[name].data_ptr())
+
+    @property
+    def _in_cur(self) -> int:
+        return self._tick.in_cur
+
+    @property
+    def d_in_raw(self) -> torch.Tensor:
+        """the packed device input copy in use (upload() copies a pinned staging set into it)"""
+        return self.d_in[self._tick.in_cur][0]
 
     def allocate(self, batch: int, k_obj: int = 3, k_pred: int = 0) -> None:
         k_obj = check_object_count(k_obj, self.max_objects)
@@ -310,7 +330,7 @@ class BatchPlanner(object):
             traj=z(((NSLOT + 1) * B, NE, 7), f32))
         t.update(t_meta)
         buf = capi.Buffers()
-        t["zone_bits"] = torch.zeros((1, 1), dtype=torch.int32, device=dev)   # replaced by _upload_zones()
+        t["zone_bits"] = torch.zeros((1, 1), dtype=torch.int32, device=dev)   # replaced by _stage_zones()
         d.k_pred = 0
         d.n_zones, d.n_zone_words = 0, (self.lattice_nodes + 31) // 32
         for name in capi.BUFFER_FIELDS:
@@ -318,11 +338,12 @@ class BatchPlanner(object):
                 setattr(buf, name, t[name].data_ptr())
         self.t, self.buf, self.dims = t, buf, d
         self._generation += 1
-        self._ticked = False
         if self._traj_base is not None:
             buf.traj_base = self._traj_base.data_ptr()
-        self._gg_planes_used = False
-        self._zones_dev = None
+        self._tick = TickState()
+        # zone keys of the last staged batch, which the next stateful tick compares with (k_stage reads and writes them);
+        # one buffer per allocation, so that captured graphs keep its address
+        self._zone_key = z((B,), torch.int64)
         self._alloc_inputs(B, k_obj, k_pred)
         self._state = None   # buffers of the stateful tick, allocated by next_tick()
         # further compact export buffers: the pipelined stream planner lets the D2H of step i overlap step i + 1
@@ -362,13 +383,10 @@ class BatchPlanner(object):
         if ax.shape != ay.shape or ax.ndim != 3 or ax.shape[:2] != (NSLOT, B) or ax.shape[2] > P:
             raise ValueError("local_gg planes must have the shape [NSLOT][B][P <= p_max]")
         self._generation += 1
-        if "gg" not in self.t:
-            self.t["gg"] = torch.ones((2, NSLOT * B, P), dtype=torch.float64, device=self.device)
         host = np.ones((2, NSLOT * B, P))
         host[0, :, :ax.shape[2]] = ax.reshape(NSLOT * B, -1)
         host[1, :, :ay.shape[2]] = ay.reshape(NSLOT * B, -1)
-        self.t["gg"].copy_(torch.from_numpy(host))
-        self.buf.gg = self.t["gg"].data_ptr()
+        self.buf.gg = self._gg_planes(self.t).copy_(torch.from_numpy(host)).data_ptr()
 
     def set_gg_map(self, ax=None, ay=None, x0: float = 0.0, y0: float = 0.0, cell: float = 1.0) -> None:
         """location dependent friction from a map of the track surface, for the whole batch: ``ax``, ``ay`` [ny][nx] =
@@ -407,11 +425,16 @@ class BatchPlanner(object):
         """buffers.gg_map and the gg planes the library fills from it (allocated with the other buffers)"""
         if self._gg_map is None or self.buf is None:
             return
-        if "gg" not in self.t:
-            self.t["gg"] = torch.ones((2, NSLOT * self.dims.batch, self.dims.p_max), dtype=torch.float64,
-                                      device=self.device)
-        self.buf.gg = self.t["gg"].data_ptr()
+        self.buf.gg = self._gg_planes(self.t).data_ptr()
         self.buf.gg_map = self._gg_map.data_ptr()
+
+    def _gg_planes(self, planes: dict) -> torch.Tensor:
+        """``planes["gg"]``: the gg planes [2][NSLOT * B][p_max] of this batch (this tick's in ``t``, the last tick's in
+        the stateful memory), created as ones on first use"""
+        if "gg" not in planes:
+            planes["gg"] = torch.ones((2, NSLOT * self.dims.batch, self.dims.p_max), dtype=torch.float64,
+                                      device=self.device)
+        return planes["gg"]
 
     def device_bytes(self) -> int:
         return int(sum(v.numel() * v.element_size() for v in self.t.values()) + self.blob.numel())
@@ -437,13 +460,45 @@ class BatchPlanner(object):
         ``vel_est`` may then be a device tensor [B]."""
         if isinstance(sc, DeviceScenarioBatch):
             vel_est = self._device_args(sc, vel_est)[0]
-            self._grow_for(sc)
-            self._stage_device(sc, vel_est)
-            return
-        self._staged_on_device = False
+        self._stage(sc, vel_est, which)
+
+    def _stage(self, sc, vel_est, which: int, tick_args: tuple = None) -> None:
+        """staging of both batch kinds: the buffers grown for the batch and the zone bitmasks, then ONE kind-specific
+        step -- a ScenarioBatch is copied into pinned staging set ``which`` (upload() copies it to the device), a
+        DeviceScenarioBatch is written into the device inputs by k_stage -- then the zone keys of the batch.
+        ``tick_args`` = (sel_action, t_const, restart) of a stateful tick: they are staged along, and the tick's zone
+        rule applies (a zone under a NEW id is a new zone object: its unblock window is evaluated at this tick,
+        OLI:155-237, GLNT:43-77)."""
+        self._grow_for(sc)
+        self._stage_zones(sc.zones)
+        ts = self._tick
+        on_device = isinstance(sc, DeviceScenarioBatch)
+        sel_action, t_const, restart = tick_args or (None, None, None)
+        zone_rule = tick_args is not None and ts.zone_key_kept
+        if not on_device:
+            self._fill_staging(sc, vel_est, which, sel_action, t_const)
+        if tick_args is not None and self.on_device_start is not None:   # the host staging ends here (timing)
+            self.on_device_start()
+        if on_device:
+            self._launch_stage(sc, vel_est, sel_action, t_const, restart, zone_rule)
+        else:
+            self._put_zone_key(sc.zone_key, zone_rule)
+            if restart is not None:   # one small H2D copy of the mask (the packed upload stays as it is)
+                self._state["restart"].copy_(torch.from_numpy(restart.astype(np.int32)).pin_memory(),
+                                             non_blocking=True)
+        self.dims.k_pred = 0 if sc.n_pred is None else self._k_pred_cap
+        ts.staged_on_device = on_device
+        ts.zone_key_kept, ts.zone_key_zero = True, sc.zone_key is None
+
+    def _grow_for(self, sc) -> None:
+        """buffers for the batch size, object slots and prediction points of a batch (see allocate: growing them
+        synchronises)"""
         kp = 0 if sc.pred is None else int(sc.pred.shape[2])
         if self.dims is None or sc.size != self.dims.batch or sc.obj.shape[1] > self.dims.k_obj or kp > self._k_pred_cap:
             self.allocate(sc.size, sc.obj.shape[1], kp)
+
+    def _fill_staging(self, sc: ScenarioBatch, vel_est, which: int, sel_action=None, t_const=None) -> None:
+        """a host batch (and the sel_action / t_const of a stateful tick) into pinned staging set ``which``"""
         if self._h2d_ev[which] is not None:   # an asynchronous upload may still read this pinned set
             self._h2d_ev[which].synchronize()
             self._h2d_ev[which] = None
@@ -459,23 +514,40 @@ class BatchPlanner(object):
         h["obj"].numpy()[:, :k, :] = sc.obj
         h["zone_sel"].numpy()[...] = -1 if sc.zone_sel is None else sc.zone_sel
         h["n_pred"].numpy()[...] = -1
-        self.dims.k_pred = 0
-        if sc.n_pred is not None:     # kp >= 1 here, so allocate() above provided the obj_pred staging
+        if sc.n_pred is not None:     # with pred, so _grow_for provided the obj_pred staging
             h["n_pred"].numpy()[:, :k] = sc.n_pred
             h["obj_pred"].numpy()[...] = 0.0
-            h["obj_pred"].numpy()[:, :k, :kp, :] = sc.pred
-            self.dims.k_pred = self._k_pred_cap
-        self._upload_zones(sc.zones)
-        self._zone_key = sc.zone_key.copy() if sc.zone_key is not None else np.zeros(sc.size, dtype=np.int64)
+            h["obj_pred"].numpy()[:, :k, :sc.pred.shape[2], :] = sc.pred
+        if sel_action is not None:
+            h["sel_action"].numpy()[...] = np.asarray(sel_action, dtype=np.int32).reshape(-1)
+            h["t_const"].numpy()[...] = np.broadcast_to(np.asarray(t_const, dtype=np.float64), (self.dims.batch,))
 
-    def _upload_zones(self, zones) -> None:
-        """zone bitmasks: bit (node_off[layer] + node) of mask z = that node is blocked by zone z (GLNT:46, 96-99)."""
-        self._zones_dev = None
+    def _put_zone_key(self, zone_key, zone_rule: bool) -> None:
+        """the zone keys of a host batch into _zone_key, where k_stage puts those of a device batch: a copy from pinned
+        memory on the stream, none while _zone_key is all zero and the batch has no keys.  zone_rule: first zone_s0[b]
+        = -1 where the new key is non-zero and differs from the last one (k_stage's rule), as a masked fill"""
+        if zone_key is None:
+            if not self._tick.zone_key_zero:
+                self._zone_key.zero_()
+            return
+        key = torch.from_numpy(np.ascontiguousarray(zone_key, dtype=np.int64)).pin_memory()
+        key = key.to(self.device, non_blocking=True)
+        if zone_rule:
+            self._state["zone_s0"].masked_fill_((key != self._zone_key) & (key != 0), -1)
+        self._zone_key.copy_(key)
+
+    def _stage_zones(self, zones) -> None:
+        """zone bitmasks: bit (node_off[layer] + node) of mask z = that node is blocked by zone z (GLNT:46, 96-99);
+        uploaded (pinned, asynchronously) only when the zone list changed"""
         if not zones:
             self.dims.n_zones = 0
             return
-        self.t["zone_bits"] = torch.from_numpy(self._zone_bits(zones)).to(self.device)
-        self.buf.zone_bits = self.t["zone_bits"].data_ptr()
+        key = tuple((np.asarray(lay).tobytes(), np.asarray(nod).tobytes()) for lay, nod in zones)
+        if key != self._tick.zones:
+            bits = torch.from_numpy(self._zone_bits(zones)).pin_memory()
+            self.t["zone_bits"] = bits.to(self.device, non_blocking=True)
+            self.buf.zone_bits = self.t["zone_bits"].data_ptr()
+            self._tick.zones = key
         self.dims.n_zones = len(zones)
 
     def _zone_bits(self, zones) -> np.ndarray:
@@ -522,17 +594,10 @@ class BatchPlanner(object):
                 arg("sel_action", sel_action, (torch.int32, torch.int64), np.int32), t_const,
                 arg("restart", restart, (torch.bool, torch.uint8, torch.int8, torch.int32, torch.int64), np.int32))
 
-    def _grow_for(self, sc: DeviceScenarioBatch) -> None:
-        """buffers for the batch size, object slots and prediction points of a device batch (see allocate: growing them
-        synchronises)"""
-        kp = 0 if sc.pred is None else int(sc.pred.shape[2])
-        if self.dims is None or sc.size != self.dims.batch or sc.obj.shape[1] > self.dims.k_obj or kp > self._k_pred_cap:
-            self.allocate(sc.size, sc.obj.shape[1], kp)
-
-    def _stage_device(self, sc: DeviceScenarioBatch, vel_est=None, sel_action=None, t_const=None, restart=None,
-                      zone_rule: bool = False) -> None:
-        """k_stage: the inputs of a device batch into the input set in use, with the bytes stage_scenarios + upload
-        write (and with sel_action those of _stage_next); zone_rule: the zone key rule of a stateful tick"""
+    def _launch_stage(self, sc: DeviceScenarioBatch, vel_est, sel_action, t_const, restart, zone_rule: bool) -> None:
+        """k_stage: the inputs of a device batch into the input copy in use, the bytes _fill_staging + upload() write
+        (with sel_action also those of a stateful tick), and its zone keys into _zone_key; zone_rule: the zone rule of
+        a stateful tick"""
         src = capi.StageSrc()
 
         def put(name, a):
@@ -549,7 +614,6 @@ class BatchPlanner(object):
         src.k_src = int(sc.obj.shape[1])
         src.kp_src = 0 if sc.pred is None else int(sc.pred.shape[2])
         src.kp_dst = self._k_pred_cap
-        self.dims.k_pred = 0 if sc.pred is None else self._k_pred_cap
         if sel_action is not None:
             put("sel_action", sel_action)
             src.sel_action_bytes = sel_action.element_size()
@@ -560,42 +624,13 @@ class BatchPlanner(object):
         if restart is not None:
             put("restart", restart)
             src.restart_bytes = restart.element_size()
-        kept = self._cross_zone_key()
-        src.zone_key_rule = int(zone_rule and kept)
-        src.zone_key_last = self._zone_key_dev.data_ptr()
-        self._stage_zones_device(sc.zones)
-        self._staged_on_device = True
+        src.zone_key_rule = int(zone_rule)
+        src.zone_key_last = self._zone_key.data_ptr()
         capi.check(self.lib, self.lib.ltpl_stage_inputs_batch(C.byref(self.dims), C.byref(self.buf), C.byref(src),
                                                               self.stream), "ltpl_stage_inputs_batch")
 
-    def _cross_zone_key(self) -> bool:
-        """the zone key of the last staging lives on the device from now on (_zone_key_dev, which k_stage reads and
-        writes); after a host staging it crosses over once.  Returns whether the last staging kept a key of this batch
-        size (the zone key rule of a stateful tick applies)."""
-        B = self.dims.batch
-        last = getattr(self, "_zone_key", None)
-        if self._zone_key_dev is None or self._zone_key_dev.shape[0] != B:
-            self._zone_key_dev = torch.zeros((B,), dtype=torch.int64, device=self.device)
-        if isinstance(last, np.ndarray) and last.shape == (B,):
-            self._zone_key_dev.copy_(torch.from_numpy(last))
-        self._zone_key = self._zone_key_dev
-        return last is not None and tuple(last.shape) == (B,)
-
-    def _stage_zones_device(self, zones) -> None:
-        """zone bitmasks of a device batch: uploaded (pinned, asynchronously) only when the zone list changed"""
-        if not zones:
-            self.dims.n_zones = 0
-            return
-        key = tuple((np.asarray(lay).tobytes(), np.asarray(nod).tobytes()) for lay, nod in zones)
-        if key != self._zones_dev:
-            bits = torch.from_numpy(self._zone_bits(zones)).pin_memory()
-            self.t["zone_bits"] = bits.to(self.device, non_blocking=True)
-            self.buf.zone_bits = self.t["zone_bits"].data_ptr()
-            self._zones_dev = key
-        self.dims.n_zones = len(zones)
-
     def upload(self, which: int = 0) -> None:
-        if self._staged_on_device:   # k_stage has already written the device inputs
+        if self._tick.staged_on_device:   # k_stage has already written the device inputs
             return
         self.d_in_raw.copy_(self.h_in_raw[which], non_blocking=True)      # one packed H2D copy
         ev = torch.cuda.Event()
@@ -644,12 +679,15 @@ class BatchPlanner(object):
         stream.synchronize()
         n = int(out["queue_cnt"][2])
         if n:
-            src = next(tb for tb in self.traj_bufs if tb.data_ptr() == self.buf.traj)   # the set the kernels wrote
-            out["traj"][:n].copy_(src[:n], non_blocking=True)
+            out["traj"][:n].copy_(self._traj_buf()[:n], non_blocking=True)
             stream.synchronize()   # the caller reads pinned host memory: the copy has to be complete
         out["n_rows"] = n
         out["incl_emerg_traj"] = bool(self.params.incl_emerg_traj)
         return out
+
+    def _traj_buf(self) -> torch.Tensor:
+        """the compact export buffer of traj_bufs that buffers.traj points at (the one the last tick wrote)"""
+        return next(tb for tb in self.traj_bufs if tb.data_ptr() == self.buf.traj)
 
     def plan_stream(self, batches, vel_est=None, device_hook=None):
         """Pipelined end-to-end planning of a sequence of ScenarioBatch objects (generator of result dicts, in order).
@@ -659,12 +697,11 @@ class BatchPlanner(object):
         next step (CUDA events for the hand-over).  With N_SETS = 3 staging / export buffer sets the host stages step
         i + 1 while the GPU runs step i and the copy engine drains step i - 1, so the GPU never waits for the host.
         Results are views of pinned host memory; a result stays valid until N_SETS - 1 further results were taken."""
-        dev = self.device
         ns = self.N_SETS
-        compute = torch.cuda.current_stream(dev)
-        copy_stream = getattr(self, "_copy_stream", None)
-        if copy_stream is None:
-            copy_stream = self._copy_stream = torch.cuda.Stream(device=dev)
+        compute = torch.cuda.current_stream(self.device)
+        if self._copy_stream is None:
+            self._copy_stream = torch.cuda.Stream(device=self.device)
+        copy_stream = self._copy_stream
         ev_meta = [torch.cuda.Event() for _ in range(ns)]
         ev_d2h = [None] * ns
         pending = []          # sets submitted, trajectory copy not yet issued
@@ -685,46 +722,39 @@ class BatchPlanner(object):
             inflight.append(k)
 
         try:
-            yield from self._plan_stream_loop(batches, vel_est, device_hook, ns, compute, ev_meta, ev_d2h, pending,
-                                              inflight, issue_copy)
-        finally:
-            self.buf.traj = self.traj_bufs[0].data_ptr()
-
-    def _plan_stream_loop(self, batches, vel_est, device_hook, ns, compute, ev_meta, ev_d2h, pending, inflight,
-                          issue_copy):
-        i = 0
-        for sc in batches:
-            k = i % ns
-            if self.dims is not None and sc.size != self.dims.batch and (pending or inflight):
-                raise ValueError("plan_stream: the batch size changed while results are in flight")
-            while inflight and (inflight[0] == k or ev_d2h[inflight[0]].query()):
-                # hand out finished results in order; the set about to be reused must have left the device first
-                j = inflight.pop(0)
+            for i, sc in enumerate(batches):
+                k = i % ns
+                if self.dims is not None and sc.size != self.dims.batch and (pending or inflight):
+                    raise ValueError("plan_stream: the batch size changed while results are in flight")
+                while inflight and (inflight[0] == k or ev_d2h[inflight[0]].query()):
+                    # hand out finished results in order; the set about to be reused must have left the device first
+                    j = inflight.pop(0)
+                    ev_d2h[j].synchronize()
+                    yield self.h_out_sets[j]
+                if isinstance(sc, DeviceScenarioBatch):
+                    raise ValueError("plan_stream overlaps the host staging of ScenarioBatch objects; plan a "
+                                     "DeviceScenarioBatch with plan_batch or tick()")
+                if device_hook is not None and hasattr(device_hook, "before"):
+                    device_hook.before(k)   # e.g. wait until a collective that still reads buffer set k has finished
+                self.stage_scenarios(sc, vel_est=vel_est, which=k)
+                self.buf.traj = self.traj_bufs[k].data_ptr()
+                self.upload(which=k)
+                self.set_startpos()
+                self.tick()
+                if device_hook is not None:     # e.g. an all-gather of the device-side action sets (multi-GPU)
+                    device_hook(k)
+                self._download_meta(k)
+                ev_meta[k].record(compute)
+                pending.append(k)
+                if len(pending) > 1:            # issue the trajectory copy of the previous step; it overlaps this step
+                    issue_copy(pending.pop(0))
+            while pending:
+                issue_copy(pending.pop(0))
+            for j in inflight:
                 ev_d2h[j].synchronize()
                 yield self.h_out_sets[j]
-            if isinstance(sc, DeviceScenarioBatch):
-                raise ValueError("plan_stream overlaps the host staging of ScenarioBatch objects; plan a "
-                                 "DeviceScenarioBatch with plan_batch or tick()")
-            if device_hook is not None and hasattr(device_hook, "before"):
-                device_hook.before(k)   # e.g. wait until a collective that still reads buffer set k has finished
-            self.stage_scenarios(sc, vel_est=vel_est, which=k)
-            self.buf.traj = self.traj_bufs[k].data_ptr()
-            self.upload(which=k)
-            self.set_startpos()
-            self.tick()
-            if device_hook is not None:     # e.g. an all-gather of the device-side action sets (multi-GPU)
-                device_hook(k)
-            self._download_meta(k)
-            ev_meta[k].record(compute)
-            pending.append(k)
-            if len(pending) > 1:            # issue the trajectory copy of the previous step; it overlaps this step
-                issue_copy(pending.pop(0))
-            i += 1
-        while pending:
-            issue_copy(pending.pop(0))
-        for j in inflight:
-            ev_d2h[j].synchronize()
-            yield self.h_out_sets[j]
+        finally:
+            self.buf.traj = self.traj_bufs[0].data_ptr()
 
     # -- kernels ---------------------------------------------------------------------------------------------------------------
     def _call(self, name):
@@ -738,8 +768,8 @@ class BatchPlanner(object):
         self._tick_count += 1
         self.params.traj_base_id = 10 * self._tick_count if self._traj_base is None else 0
         self._call(name)
-        self._gg_planes_used = self.buf.gg is not None
-        self._ticked = True
+        self._tick.gg_planes_used = self.buf.gg is not None
+        self._tick.ticked = True
 
     def set_startpos(self) -> None:
         self._call("ltpl_set_startpos_batch")
@@ -772,6 +802,7 @@ class BatchPlanner(object):
                   st_info=z((B, 8), i32), vel_plan=z((B,), f64), course=z((B, self.dims.n_export), f64),
                   obj_dist=z((B,), f64))
         st["zone_s0"] = torch.full((B,), -1, dtype=i32, device=dev)
+        st["restart"] = z((B,), i32)   # buffers.restart of the ticks with a restart mask
         self.buf.zone_s0 = st["zone_s0"].data_ptr()
         self.buf.trim = t["trim"].data_ptr()
         self._state = st
@@ -787,46 +818,22 @@ class BatchPlanner(object):
         mask = mask.astype(bool)
         return mask if mask.any() else None
 
-    def _stage_restart(self, mask) -> None:
-        """buffers.restart: NULL without restarts; else its own small H2D copy (the packed input upload stays as it is)"""
-        if mask is None:
-            self.buf.restart = None
-            return
-        st = self._state
-        self._restart_buffer()
-        if st["restart_ev"] is not None:      # the last copy may still read the pinned staging
-            st["restart_ev"].synchronize()
-        st["h_restart"].numpy()[...] = mask
-        st["restart"].copy_(st["h_restart"], non_blocking=True)
-        st["restart_ev"] = torch.cuda.Event()
-        st["restart_ev"].record(torch.cuda.current_stream(self.device))
-        self.buf.restart = st["restart"].data_ptr()
-
-    def _restart_buffer(self) -> torch.Tensor:
-        """buffers.restart of the stateful tick ([B] int32 on the device) with its pinned staging"""
-        st = self._state
-        if "restart" not in st:
-            st["restart"] = torch.zeros((self.dims.batch,), dtype=torch.int32, device=self.device)
-            st["h_restart"] = torch.zeros((self.dims.batch,), dtype=torch.int32).pin_memory()
-            st["restart_ev"] = None
-        return st["restart"]
-
     def _stage_next(self, sc, sel_action, t_const, vel_est, restart=None) -> None:
-        """host side of a stateful tick: pointer swaps, the host memcpy into the pinned staging set, ONE packed H2D copy
-        (scenario arrays incl. sel_action / t_const) and ONE device copy (the small per-path arrays of the last tick);
-        with restarts one more small H2D copy (the mask).  A DeviceScenarioBatch replaces the memcpy, the uploads and the
-        host zone-key comparison by one k_stage launch."""
+        """host side of a stateful tick: pointer swaps, ONE device copy (the small per-path arrays of the last tick),
+        then the staging of stage_scenarios into the other input copy with sel_action / t_const and the restart mask.
+        A ScenarioBatch: host memcpy into the pinned staging set and ONE packed H2D copy, with restarts one more small
+        H2D copy (the mask).  A DeviceScenarioBatch: one k_stage launch."""
         if sc.size != self.dims.batch:
             raise ValueError("stateful tick: the batch size must not change within a session (re-anchor with "
                              "set_startpos on a new batch, or restart single scenarios with `restart`)")
-        on_device = isinstance(sc, DeviceScenarioBatch)
-        if on_device:   # before the swaps below: refused inputs change nothing
-            if sel_action is None or t_const is None:
-                raise ValueError("stateful tick: sel_action and t_const are required")
-            dev_args = self._device_args(sc, vel_est, sel_action, t_const, restart)
+        # before the swaps below: refused inputs change nothing
+        if sel_action is None or t_const is None:
+            raise ValueError("stateful tick: sel_action and t_const are required")
+        if isinstance(sc, DeviceScenarioBatch):
+            vel_est, sel_action, t_const, restart = self._device_args(sc, vel_est, sel_action, t_const, restart)
         else:
-            check_object_count(sc.obj.shape[1], self.max_objects)   # before the swaps below: a refused list changes nothing
-            mask = self._restart_mask(restart)                       # (likewise)
+            check_object_count(sc.obj.shape[1], self.max_objects)
+            restart = self._restart_mask(restart)
         if self._state is None:
             self._alloc_state()
         st, t, buf = self._state, self.t, self.buf
@@ -839,61 +846,26 @@ class BatchPlanner(object):
         for k in self._SMALL:
             setattr(buf, "prev_" + k, st["prev_small"][k].data_ptr())
         # location dependent local_gg of the last tick = backup for a brake on the old plan (__backup_path_gg, OTH:970)
-        if self._gg_planes_used:
-            if "gg" not in st["other"]:
-                st["other"]["gg"] = torch.ones_like(t["gg"])
-            t["gg"], st["other"]["gg"] = st["other"]["gg"], t["gg"]
+        if self._tick.gg_planes_used:
+            t["gg"], st["other"]["gg"] = self._gg_planes(st["other"]), t["gg"]
             buf.prev_gg = st["other"]["gg"].data_ptr()
         else:
             buf.prev_gg = None
         buf.gg = None            # this tick's local_gg arrives with its calc_vel_profile ...
         self._bind_gg_map()      # ... or from the friction map, into this tick's planes
-        if on_device:
-            self._stage_next_device(sc, dev_args)
-            return
-        # a zone under a NEW id is a new zone object: its unblock window is evaluated at this tick (OLI:155-237, GLNT:43-77)
-        zkey = sc.zone_key if sc.zone_key is not None else np.zeros(sc.size, dtype=np.int64)
-        last = getattr(self, "_zone_key", None)               # of the batch staged for the previous tick
-        if isinstance(last, torch.Tensor):                    # staged from a device batch: crosses over once
-            last = last.cpu().numpy()
-        if last is not None and last.shape == zkey.shape:
-            changed = np.nonzero((zkey != last) & (zkey != 0))[0]
-            if changed.size:
-                st["zone_s0"][torch.as_tensor(changed, device=self.device)] = -1
         # pos_est of the previous calc_vel_profile (OTH:537) = `pos` of the input copy the last tick used; this tick
-        # uploads into the other copy (a batch with more objects than before re-creates only the input buffers)
-        self._pos_last = t["pos"]
-        self.stage_scenarios(sc, vel_est=vel_est)
-        self._use_inputs(1 - self._in_cur)
-        buf.pos_last = self._pos_last.data_ptr()
-        for k in ("st_info", "vel_plan", "course", "obj_dist"):
-            setattr(buf, k, st[k].data_ptr())
-        buf.sel_action = t["sel_action"].data_ptr()
-        buf.t_const = t["t_const"].data_ptr()
-        self.h_in["sel_action"].numpy()[...] = np.asarray(sel_action, dtype=np.int32).reshape(-1)
-        self.h_in["t_const"].numpy()[...] = np.broadcast_to(np.asarray(t_const, dtype=np.float64), (self.dims.batch,))
-        if self.on_device_start is not None:   # measurement hook: the host staging ends here, the device work begins
-            self.on_device_start()
-        self.upload()
-        self._stage_restart(mask)
-
-    def _stage_next_device(self, sc: DeviceScenarioBatch, dev_args) -> None:
-        """_stage_next of a device batch behind the swaps: the other input copy, then k_stage (inputs, sel_action,
-        t_const, restart mask and the zone key rule)"""
-        st, t, buf = self._state, self.t, self.buf
-        self._pos_last = t["pos"]
+        # stages into the other copy (a batch with more objects than before re-creates only the input buffers)
+        self._tick.pos_last = t["pos"]
         self._grow_for(sc)
-        self._use_inputs(1 - self._in_cur)
-        buf.pos_last = self._pos_last.data_ptr()
+        self._use_inputs(1 - self._tick.in_cur)
+        buf.pos_last = self._tick.pos_last.data_ptr()
         for k in ("st_info", "vel_plan", "course", "obj_dist"):
             setattr(buf, k, st[k].data_ptr())
         buf.sel_action = t["sel_action"].data_ptr()
         buf.t_const = t["t_const"].data_ptr()
-        vel_est, sel_action, t_const, restart = dev_args
-        buf.restart = None if restart is None else self._restart_buffer().data_ptr()
-        if self.on_device_start is not None:
-            self.on_device_start()
-        self._stage_device(sc, vel_est, sel_action, t_const, restart, zone_rule=True)
+        buf.restart = None if restart is None else st["restart"].data_ptr()
+        self._stage(sc, vel_est, 0, (sel_action, t_const, restart))
+        self.upload()   # a ScenarioBatch: ONE packed H2D copy (k_stage has written a DeviceScenarioBatch)
 
     def next_calc_paths(self, sc: ScenarioBatch, sel_action, t_const, vel_est=None, restart=None) -> None:
         """calc_paths of a stateful tick (OTH:289-516 with the iterative memory): ``sc`` carries the object
@@ -946,8 +918,8 @@ class BatchPlanner(object):
 
     def _prepare_capture(self, inputs, stateful: bool) -> None:
         """everything a tick of these inputs could allocate, grow or copy from the host, done before a capture: the
-        buffers for the batch, the memory buffers a stateful tick creates on first use, the zone key crossing over from
-        a host staging, the zone bitmasks, the id counter and the kernels' attributes (ltpl_prepare_batch)"""
+        buffers for the batch, the memory buffers a stateful tick creates on first use, the zone bitmasks, the id
+        counter and the kernels' attributes (ltpl_prepare_batch)"""
         sc = inputs.sc
         pos = self.t["pos"] if stateful else None
         self._grow_for(sc)
@@ -959,15 +931,9 @@ class BatchPlanner(object):
         if stateful:
             if self._state is None:
                 self._alloc_state()
-            if inputs.restart is not None:
-                self._restart_buffer()
-            if "gg" in self.t and "gg" not in self._state["other"]:   # what the first gg swap would create
-                self._state["other"]["gg"] = torch.ones_like(self.t["gg"])
-        if getattr(self, "_zone_key", None) is not None:
-            self._cross_zone_key()
-        elif self._zone_key_dev is None or self._zone_key_dev.shape[0] != self.dims.batch:
-            self._zone_key_dev = torch.zeros((self.dims.batch,), dtype=torch.int64, device=self.device)
-        self._stage_zones_device(sc.zones)
+            if "gg" in self.t:   # what the first gg swap would create
+                self._gg_planes(self._state["other"])
+        self._stage_zones(sc.zones)
         if self._traj_base is None:   # the ids an all-eager session would give next
             self._traj_base = torch.full((1,), 10 * self._tick_count, dtype=torch.int32, device=self.device)
         self.buf.traj_base = self._traj_base.data_ptr()
@@ -975,15 +941,12 @@ class BatchPlanner(object):
         capi.check(self.lib, self.lib.ltpl_prepare_batch(self.handle, C.byref(self.params), C.byref(self.dims),
                                                          C.byref(self.buf)), "ltpl_prepare_batch")
 
-    _TICK_ATTRS = ("_in_cur", "d_in_raw", "_pos_last", "_gg_planes_used", "_zone_key", "_zones_dev",
-                   "_staged_on_device", "_ticked")
-
     def _host_state(self) -> dict:
         """what a tick changes on the host: the pointer fields and dims a call passes, the buffer dicts (by reference)
-        and the host mirrors"""
+        and the TickState record"""
         return dict(buf=capi.Buffers.from_buffer_copy(self.buf), dims=capi.Dims.from_buffer_copy(self.dims),
                     t=dict(self.t), other=None if self._state is None else dict(self._state["other"]),
-                    attrs={k: getattr(self, k, None) for k in self._TICK_ATTRS})
+                    tick=replace(self._tick))
 
     def _set_host_state(self, hs: dict) -> None:
         C.memmove(C.addressof(self.buf), C.addressof(hs["buf"]), C.sizeof(capi.Buffers))
@@ -993,14 +956,13 @@ class BatchPlanner(object):
         if hs["other"] is not None:
             self._state["other"].clear()
             self._state["other"].update(hs["other"])
-        for k, v in hs["attrs"].items():
-            setattr(self, k, v)
+        self._tick = replace(hs["tick"])   # a copy: the record in hs serves every replay of its graph
 
     def _tick_key(self, stateful: bool) -> tuple:
         """the buffers the next tick would use: the input copy, the ping-pong planes, the gg planes and, for a stateful
         tick, whether the last velocity call ran with planes (it decides the gg swap and prev_gg)"""
-        key = (self._in_cur,) + tuple(self.t[k].data_ptr() if k in self.t else 0 for k in self._BIG + ("gg",))
-        return key + (self._gg_planes_used,) if stateful else key
+        key = (self._tick.in_cur,) + tuple(self.t[k].data_ptr() if k in self.t else 0 for k in self._BIG + ("gg",))
+        return key + (self._tick.gg_planes_used,) if stateful else key
 
     def launch_count(self) -> int:
         return int(self.lib.ltpl_launch_count())
@@ -1016,7 +978,7 @@ class BatchPlanner(object):
         The views are valid until the next tick: it rewrites these buffers, and a stateful tick swaps planes by pointer,
         so read or clone what is needed before staging the next tick."""
         out = {n: self.t[n] for n in self.DEVICE_RESULTS}
-        out["traj"] = next(tb for tb in self.traj_bufs if tb.data_ptr() == self.buf.traj)
+        out["traj"] = self._traj_buf()
         return out
 
     # -- result access (device -> host, test / facade use) ----------------------------------------------------------------------

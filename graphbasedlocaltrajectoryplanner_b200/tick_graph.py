@@ -16,7 +16,6 @@ from __future__ import annotations
 
 from dataclasses import dataclass, replace
 
-import numpy as np
 import torch
 
 from .scenarios import DeviceScenarioBatch
@@ -98,18 +97,14 @@ class TickGraph(object):
     def replay(self) -> None:
         """one tick from the current graph inputs, on the current stream: a graph launch plus the host side of the tick
         (pointer swaps, tick count); no host synchronisation, no host memory read by the device, no library call.
-        Refused with ValueError, changing nothing, on a closed or stale graph, after a tick that staged a host
-        ScenarioBatch (its zone key is on the host), or when the planner's buffers are in a state no graph was captured
-        in."""
+        Refused with ValueError, changing nothing, on a closed or stale graph, or when the planner's buffers are in a
+        state no graph was captured in."""
         pl = self.planner
         if self._entries is None:
             raise ValueError("TickGraph.replay: the graph was closed")
         if pl._generation != self._generation:
             raise ValueError("TickGraph.replay: the planner changed since the capture (allocate, set_vel_params, "
                              "set_gg_map, set_local_gg_planes, set_subbatches or grown input buffers); capture anew")
-        if isinstance(getattr(pl, "_zone_key", None), np.ndarray):
-            raise ValueError("TickGraph.replay: the last tick staged a host ScenarioBatch, whose zone keys are on the "
-                             "host; plan one tick from a DeviceScenarioBatch first")
         entry = self._entries.get(pl._tick_key(self.stateful))
         if entry is None:
             raise ValueError("TickGraph.replay: the planner's buffers are in a state this graph was not captured in "
@@ -152,7 +147,7 @@ def capture(pl, stateful: bool, sc, vel_est=None, sel_action=None, t_const=None,
         raise ValueError("%s: uploaded local_gg planes (set_local_gg_planes) are per-tick host data; a friction map "
                          "(set_gg_map) is evaluated inside the tick" % what)
     if stateful:
-        if not pl._ticked:
+        if not pl._tick.ticked:
             raise ValueError("%s: no previous tick in this session (capture_tick or tick first)" % what)
         if sc.size != pl.dims.batch:
             raise ValueError("%s: batch of %d scenarios, the session has %d" % (what, sc.size, pl.dims.batch))

@@ -215,10 +215,12 @@ def test_friction_map_closed_loop_replays_equal_eager_loop():
 
 
 # ---- parity, interleaving, ids -------------------------------------------------------------------------------------
-@pytest.mark.parametrize("shift", [0, 1])
-def test_eager_ticks_and_replays_interleave(shift):
+@pytest.mark.parametrize("shift,host", [(0, False), (1, False), (1, True)], ids=["0", "1", "1-host"])
+def test_eager_ticks_and_replays_interleave(shift, host):
     """eager, replay, replay, eager, replay after `shift` eager stateful ticks (the graph captured at either parity) ==
-    the all-eager loop, results and memory every tick; the ids count on without a gap or a repeat"""
+    the all-eager loop, results and memory every tick; the ids count on without a gap or a repeat.  host: the
+    capturing planner's eager ticks, the first one included, take the host ScenarioBatch and NumPy arguments (zones
+    and zone keys included), so replays and captures follow ticks staged from the host"""
     g = H.golden("ticks_multitick_ext_default.npz")
     n_seq = g["dt"].shape[0]
     lat = H.lattice_for("default")
@@ -232,14 +234,16 @@ def test_eager_ticks_and_replays_interleave(shift):
         dsc = sc.to_device(DEV)
         args, kw = (_dev(sel, np.int64), _dev(t_c)), dict(vel_est=_dev(v_est))
         if how == "first":
-            for pl in (pe, pg):
-                D.first_tick(pl, dsc, vel_est=kw["vel_est"])
+            D.first_tick(pe, dsc, vel_est=kw["vel_est"])
+            D.first_tick(pg, *((sc, v_est) if host else (dsc, kw["vel_est"])))
             continue
         pe.next_tick(dsc, *args, **kw)
         if graph is None and k == 1 + shift:
             graph = pg.capture_next_tick(dsc, *args, **kw)
             assert graph.n_graphs == 2
-        if how == "eager":
+        if how == "eager" and host:
+            pg.next_tick(sc, sel, t_c, vel_est=v_est)
+        elif how == "eager":
             pg.next_tick(dsc, *args, **kw)
         else:
             graph.inputs.copy_(dsc, *args, **kw)
