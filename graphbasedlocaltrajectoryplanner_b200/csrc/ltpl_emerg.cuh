@@ -8,7 +8,7 @@
 // trajectory (LTPL:401-406).
 //
 // One WARP per scenario, launched after k_export: lanes stage s and kappa of the first n_export + 1 points in shared
-// memory, lane 0 runs the brake recurrence in w = v^2 (same arithmetic as brake_profile_w), all lanes write the fp32 row
+// memory, lane 0 runs the brake recurrence in w = v^2 (brake_step, ltpl_vel.cuh), all lanes write the fp32 row
 // into the next free row of the compact export buffer (queue_cnt[2]); the f64 velocities also go to em_vx (stateful ticks:
 // get_ref_idx reads them when the caller executes this trajectory, OTH:307-309 / 518-601).
 #pragma once
@@ -70,9 +70,9 @@ k_emergency(const __grid_constant__ LtplParams prm, const __grid_constant__ Ltpl
         #pragma unroll 1
         for (int i = 0; i + 1 < m; ++i) {
             if (!stopped) {
-                const double a = ggr ? acc_brake(w, sk[i], ggr[i], 1.0 / ggr[pplane + i], 1.0, dmq)
-                                     : acc_brake(w, sk[i], prm.gg_ax, inv_ay, 1.0, dmq);
-                const double nx = fma(2.0 * a, ss[i + 1] - ss[i], w);
+                const double ds = ss[i + 1] - ss[i];
+                const double nx = ggr ? brake_step(w, sk[i], ggr[i], 1.0 / ggr[pplane + i], 1.0, dmq, ds)
+                                      : brake_step(w, sk[i], prm.gg_ax, inv_ay, 1.0, dmq, ds);
                 if (nx < 0.0) {   // tph.calc_vel_profile_brake: negative radicand -> the rest of the profile stays 0
                     stopped = true;
                     w = 0.0;

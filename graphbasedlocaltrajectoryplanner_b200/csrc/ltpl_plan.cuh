@@ -207,11 +207,39 @@ __device__ __forceinline__ bool zone_unblocked(int l, int s0, int L) {
     return (l >= s0 && l < L) || (l >= 0 && l < ((s0 + n) % (L - 1) - 1));
 }
 
+// Relaxation of the in-edge e (record r) of a node with igraph's tie rule: strict <, then the smaller dist[src]; an equal
+// pair (alt, dist[src]) sets tie.  dcur: dist of the layer before; mask (NULL: none): blocked edges of the planning window,
+// bit e + moff.  best / best_ds / best_k: the node's running minimum, its dist[src] and its predecessor.
+template <bool COSTF>
+__device__ __forceinline__ void dp_relax(const LtplEdgeRec& r, int e, const double* dcur, const unsigned* mask, int moff,
+                                         const DpCtx& c, double& best, double& best_ds, int& best_k, int& tie) {
+    const double ds = dcur[r.src];
+    if (!(ds < LTPL_INF)) return;
+    if (mask) {
+        const int idx = e + moff;
+        if ((mask[idx >> 5] >> (idx & 31)) & 1u) return;
+    }
+    double cost = r.cost;
+    if (COSTF) {   // offline_cost *= factor on this tick's copy of the planning range (GB:505-508)
+        if (e == c.fe0) cost = __dmul_rn(cost, c.ff0);
+        else if (e == c.fe1) cost = __dmul_rn(cost, c.ff1);
+        else if (e == c.fe2) cost = __dmul_rn(cost, c.ff2);
+    }
+    const double alt = __dadd_rn(ds, cost);
+    if (alt < best || (alt == best && ds < best_ds)) {
+        best = alt;
+        best_ds = ds;
+        best_k = r.src;
+    } else if (alt == best && ds == best_ds) {
+        tie = 1;
+    }
+}
+
 // Runs the layer transitions li_begin .. n_steps; returns the number of completed steps (last layer with a reachable
 // node).  li_begin == 1 starts at start_node; li_begin > 1 resumes from the snapshot in c.dsave (the pred rows below
 // li_begin are those of the run that took the snapshot).  After step snap_at the state is saved to c.dsave.
-// Each lane owns one node of the next layer and scans its in-edges IN CSC ORDER, which keeps igraph's relaxation order
-// and tie rule (strict <, then smaller dist[src]) bit for bit.
+// Each lane owns one node of the next layer and relaxes its in-edges IN CSC ORDER, which keeps igraph's relaxation order
+// and tie rule bit for bit.
 // DENSE: lattices with several in-edges per node keep two edge records in flight (6 % on the shipped lattice); sparse ones
 // (mostly 0 or 1 in-edge: the "216 x 11" / "430 x 21" parameter sets) run the plain loop, which is faster there
 template <bool ZONE, bool COSTF = false, bool DENSE = false>
@@ -252,38 +280,17 @@ __device__ __forceinline__ int dp_run(const LatDev& lt, int lane, DpCtx& c, int 
             if (ZONE && present && zs) present = !((zs[(nbase + j) >> 5] >> ((nbase + j) & 31)) & 1u);
             if (present) {
                 const int2 io = lt.in_off[nbase + j];
-                auto relax = [&](const LtplEdgeRec& r, int e) {
-                    const double ds = dcur[r.src];
-                    if (!(ds < LTPL_INF)) return;
-                    if (mask) {
-                        const int idx = e + moff;
-                        if ((mask[idx >> 5] >> (idx & 31)) & 1u) return;
-                    }
-                    double cost = r.cost;
-                    if (COSTF) {   // offline_cost *= factor on this tick's copy of the planning range (GB:505-508)
-                        if (e == c.fe0) cost = __dmul_rn(cost, c.ff0);
-                        else if (e == c.fe1) cost = __dmul_rn(cost, c.ff1);
-                        else if (e == c.fe2) cost = __dmul_rn(cost, c.ff2);
-                    }
-                    const double alt = __dadd_rn(ds, cost);
-                    if (alt < best || (alt == best && ds < best_ds)) {
-                        best = alt;
-                        best_ds = ds;
-                        best_k = r.src;
-                    } else if (alt == best && ds == best_ds) {
-                        tie = 1;
-                    }
-                };
                 // in-edges in CSC order (igraph's relaxation order); nodes with many in-edges keep two records in flight
                 int k = 0;
                 #pragma unroll 1
                 for (; DENSE && k + 1 < io.y; k += 2) {
                     const LtplEdgeRec ra = lt.edge_rec[io.x + k], rb = lt.edge_rec[io.x + k + 1];
-                    relax(ra, io.x + k);
-                    relax(rb, io.x + k + 1);
+                    dp_relax<COSTF>(ra, io.x + k, dcur, mask, moff, c, best, best_ds, best_k, tie);
+                    dp_relax<COSTF>(rb, io.x + k + 1, dcur, mask, moff, c, best, best_ds, best_k, tie);
                 }
                 #pragma unroll 1
-                for (; k < io.y; ++k) relax(lt.edge_rec[io.x + k], io.x + k);
+                for (; k < io.y; ++k)
+                    dp_relax<COSTF>(lt.edge_rec[io.x + k], io.x + k, dcur, mask, moff, c, best, best_ds, best_k, tie);
             }
             dnxt[j] = best;
             c.pred[li * maxn + j] = (unsigned char)best_k;
@@ -342,28 +349,8 @@ __device__ __forceinline__ int dp_run_pair(const LatDev& lt, int lane, DpCtx& c,
             const int2 io = lt.in_off[nbase + j];
             #pragma unroll 1
             for (int k = 0; k < io.y; ++k) {
-                const int e = io.x + k;
-                const LtplEdgeRec r = lt.edge_rec[e];
-                const double ds = dcur[r.src];
-                if (!(ds < LTPL_INF)) continue;
-                if (mask) {
-                    const int idx = e + moff;
-                    if ((mask[idx >> 5] >> (idx & 31)) & 1u) continue;
-                }
-                double cost = r.cost;
-                if (COSTF) {
-                    if (e == c.fe0) cost = __dmul_rn(cost, c.ff0);
-                    else if (e == c.fe1) cost = __dmul_rn(cost, c.ff1);
-                    else if (e == c.fe2) cost = __dmul_rn(cost, c.ff2);
-                }
-                const double alt = __dadd_rn(ds, cost);
-                if (alt < best || (alt == best && ds < best_ds)) {
-                    best = alt;
-                    best_ds = ds;
-                    best_k = r.src;
-                } else if (alt == best && ds == best_ds) {
-                    tie = 1;
-                }
+                const LtplEdgeRec r = lt.edge_rec[io.x + k];
+                dp_relax<COSTF>(r, io.x + k, dcur, mask, moff, c, best, best_ds, best_k, tie);
             }
         }
         dnxt[j] = best;

@@ -451,10 +451,10 @@ k_backup(const __grid_constant__ LtplParams prm, const __grid_constant__ LtplDim
             double wn = 0.0;
             if (i + 1 < n_p) {
                 if (!stopped) {
-                    const double a =
-                        ggr.p ? acc_brake(w, fabs(K[i]), ggr(GG_AX, i), 1.0 / ggr(GG_AY, i), prm.dyn_model_exp, dmq)
-                              : acc_brake(w, fabs(K[i]), prm.gg_ax, inv_ay, prm.dyn_model_exp, dmq);
-                    const double nx = fma(2.0 * a, E[i], w);
+                    const double kabs = fabs(K[i]), ds = E[i];
+                    const double nx =
+                        ggr.p ? brake_step(w, kabs, ggr(GG_AX, i), 1.0 / ggr(GG_AY, i), prm.dyn_model_exp, dmq, ds)
+                              : brake_step(w, kabs, prm.gg_ax, inv_ay, prm.dyn_model_exp, dmq, ds);
                     if (nx < 0.0)
                         stopped = true;
                     else

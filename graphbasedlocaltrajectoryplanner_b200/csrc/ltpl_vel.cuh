@@ -27,6 +27,12 @@ __device__ __forceinline__ double acc_tire(double w, double kabs, double ax_max,
 __device__ __forceinline__ double acc_brake(double w, double kabs, double ax_max, double inv_ay, double exp_, double dm) {
     return fma(-w, dm, -acc_tire(w, kabs, ax_max, inv_ay, exp_));
 }
+// one step of a brake profile (tph.calc_vel_profile_brake) over ds: w_next = w + 2 acc_brake(w) ds, unclamped.  A negative
+// value is a negative radicand; what standstill means is left to the caller.
+__device__ __forceinline__ double brake_step(double w, double kabs, double ax_max, double inv_ay, double exp_, double dm,
+                                             double ds) {
+    return fma(2.0 * acc_brake(w, kabs, ax_max, inv_ay, exp_, dm), ds, w);
+}
 
 #define LTPL_WARPS_PER_CTA_EXPORT 8
 

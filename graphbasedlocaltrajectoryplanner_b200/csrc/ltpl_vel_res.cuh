@@ -130,12 +130,93 @@ __device__ __forceinline__ float vr_tire(const VRCfg& c, float w, float K, float
     return vr_tire_pow(w * K, ax, c.exp_, c.inv_exp);
 }
 
-// Forward sweep of one lane's profile on points [lo, hi] of its path (K, E2, W: the path's shared-memory rows):
-// tph.__solver_fb_acc_profile(backwards=False): start value min(curvature limit, wcap), acceleration phases from the
-// rising edges of the curvature-limit profile, end clamp we (< 0: none).  The step is branch-free (selects).  The
-// machine limit is a table segment cached in registers; v moves slowly, and when a lane leaves its segment the WHOLE
-// warp takes one step to the neighbouring segment (warp-uniform branch: a miss never serialises lanes).
-// (pure brake profiles: vr_brake below)
+// Machine limit at v: the table segment is cached in registers (a sweep loads segment 1 first).  v moves slowly, and when
+// a lane leaves its segment the WHOLE warp takes one step to the neighbouring segment (warp-uniform branch: a miss never
+// serialises lanes).  Every lane of the warp calls find; need: the lane uses the result.
+struct VRSeg {
+    int sg;
+    float xlo, xhi, x0, f0, sl;
+    __device__ __forceinline__ void load(const VRCfg& c, int s) {
+        sg = s;
+        xlo = c.xl[s];
+        xhi = c.xl[s + 1];
+        x0 = c.x0[s];
+        f0 = c.f0[s];
+        sl = c.sl[s];
+    }
+    __device__ __forceinline__ float find(const VRCfg& c, float v, bool need) {
+        bool miss = need && !(v >= xlo && v < xhi);
+        while (__any_sync(LTPL_FULL, miss)) {
+            load(c, miss ? sg + ((v >= xhi) ? 1 : -1) : sg);
+            miss = need && !(v >= xlo && v < xhi);
+        }
+        return fmaf(sl, v - x0, f0);
+    }
+};
+
+// start value of a forward sweep: min(curvature limit 1 / K'[0], w_max, w_cap)
+__device__ __forceinline__ float vr_w_start(float k0, float wmax, float wcap) {
+    return fminf(fminf(vr_rcp(k0), wmax), wcap);
+}
+// end clamp of a profile: v[-1] = min(v[-1], v_end)
+__device__ __forceinline__ void vr_clamp_end(float& w, float we) {
+    if (w > we) w = we;
+}
+
+// One lane's sweep of tph.__solver_fb_acc_profile at its last point: w, K', longitudinal tyre limit and limit profile o
+// there, and the acceleration phases (a phase starts at a rising edge of o and ends where the integrated w exceeds
+// w_max; outside a phase the profile is o itself).  A new sweep starts outside a phase.  The steps are branch-free
+// (selects).
+struct VRSweep {
+    float cur, k_prev, ax_prev, o_prev;
+    bool prev_rise = false, active = false;
+    __device__ __forceinline__ void start(float w0, float k0, float ax0) {
+        cur = w0;
+        o_prev = w0;
+        k_prev = k0;
+        ax_prev = ax0;
+    }
+    // backwards=False, mode 'accel_forw': to the next point (K' kq, tyre limit axq; e2 = 2 el between the points), limit
+    // profile = curvature limit; live: the lane uses the result (the machine limit is only looked up for those lanes)
+    template <bool EXP1>
+    __device__ __forceinline__ float fwd(const VRCfg& c, VRSeg& seg, float kq, float axq, float e2, float wmax, bool live) {
+        const float o_n = fminf(vr_rcp(kq), wmax);
+        const bool rise = o_n > o_prev;
+        active = active || (rise && !prev_rise);
+        const float v = vr_sqrt(fmaxf(cur, 0.0f));
+        const float a_m = seg.find(c, v, live && active);   // machine limit: only inside an acceleration phase
+        const float a_t = vr_tire<EXP1>(c, cur, k_prev, ax_prev);
+        const float a = fmaf(-cur, c.dm, fminf(a_t, a_m));   // min(tyre, machine(v)) + drag
+        const float wn = fmaf(a, e2, cur);
+        return advance(wn, o_n, kq, axq, wmax, rise);
+    }
+    // flipped arrays, mode 'decel_backw' with one look-ahead correction: to the next point in the flipped order (K' kq,
+    // tyre limit axq, limit profile o_n = the forward profile there; e2 = 2 el between the points)
+    template <bool EXP1>
+    __device__ __forceinline__ float bwd(const VRCfg& c, float o_n, float kq, float axq, float e2, float wmax) {
+        const bool rise = o_n > o_prev;
+        active = active || (rise && !prev_rise);
+        const float a = fmaf(cur, c.dm, vr_tire<EXP1>(c, cur, k_prev, ax_prev));
+        float wn = fmaf(a, e2, cur);
+        const float a2 = fmaf(wn, c.dm, vr_tire<EXP1>(c, wn, kq, axq));
+        wn = fminf(wn, fmaf(a2, e2, cur));
+        return advance(wn, o_n, kq, axq, wmax, rise);
+    }
+    // both directions: w at the next point from the integrated wn (inside a phase) or the limit o_n, and the phase's end
+    __device__ __forceinline__ float advance(float wn, float o_n, float kq, float axq, float wmax, bool rise) {
+        const float nxt = active ? fminf(wn, o_n) : o_n;
+        active = active && !(wn > wmax);
+        cur = nxt;
+        prev_rise = rise;
+        o_prev = o_n;
+        k_prev = kq;
+        ax_prev = axq;
+        return nxt;
+    }
+};
+
+// Forward sweep of one lane's profile on points [lo, hi] of its path (K, E2, W: the path's shared-memory rows), end
+// clamp we (< 0: none).  (pure brake profiles: vr_brake below)
 // GG: per-point longitudinal tyre limit AX[] (location dependent local_gg), else the constant c.ax_max
 template <bool EXP1, bool GG>
 __device__ __noinline__ void vr_forward(const VRCfg c, bool on, const float* __restrict__ K,
@@ -147,49 +228,21 @@ __device__ __noinline__ void vr_forward(const VRCfg c, bool on, const float* __r
     for (int o = 16; o > 0; o >>= 1) lmax = max(lmax, __shfl_xor_sync(LTPL_FULL, lmax, o));
     if (lmax < 0) return;
     if (len < 0) lo = 0;
-    float k_prev = K[lo], ax_prev = GG ? AX[lo] : c.ax_max;
-    float cur = fminf(fminf(vr_rcp(k_prev), wmax), wcap);
-    if (len >= 0) W[lo] = cur;
-    float o_prev = cur;
-    bool prev_rise = false, active = false;
-    int sg = 1;   // cached table segment
-    float xlo = c.xl[1], xhi = c.xl[2], x0 = c.x0[1], f0 = c.f0[1], sl = c.sl[1];
+    VRSweep s;
+    s.start(vr_w_start(K[lo], wmax, wcap), K[lo], GG ? AX[lo] : c.ax_max);
+    if (len >= 0) W[lo] = s.cur;
+    VRSeg seg;
+    seg.load(c, 1);
     // lanes whose profile has ended keep stepping on clamped indices without storing: no select in the step needs `live`
     const int pcap = nmax - 1;
 #pragma unroll 2
     for (int i = 1; i <= lmax; ++i) {
         const bool live = i <= len;
         const int p = min(lo + i, pcap);
-        const float kq = K[p], e2 = E2[p - 1];
-        const float o_n = fminf(vr_rcp(kq), wmax);
-        const bool rise = o_n > o_prev;
-        active = active || (rise && !prev_rise);
-        const float v = vr_sqrt(fmaxf(cur, 0.0f));
-        const bool need = live && active;   // machine limit: only inside an acceleration phase
-        bool miss = need && !(v >= xlo && v < xhi);
-        while (__any_sync(LTPL_FULL, miss)) {
-            if (miss) sg += (v >= xhi) ? 1 : -1;
-            xlo = c.xl[sg];
-            xhi = c.xl[sg + 1];
-            x0 = c.x0[sg];
-            f0 = c.f0[sg];
-            sl = c.sl[sg];
-            miss = need && !(v >= xlo && v < xhi);
-        }
-        const float a_t = vr_tire<EXP1>(c, cur, k_prev, ax_prev);
-        const float a_m = fmaf(sl, v - x0, f0);                              // mode 'accel_forw': min(tyre, machine(v))
-        const float a = fmaf(-cur, c.dm, fminf(a_t, a_m));                   // + drag
-        const float wn = fmaf(a, e2, cur);
-        const float nxt = active ? fminf(wn, o_n) : o_n;
-        active = active && !(wn > wmax);
-        if (live) W[p] = nxt;
-        cur = nxt;
-        prev_rise = rise;
-        o_prev = o_n;
-        k_prev = kq;
-        if (GG) ax_prev = AX[p];
+        const float w = s.fwd<EXP1>(c, seg, K[p], GG ? AX[p] : c.ax_max, E2[p - 1], wmax, live);
+        if (live) W[p] = w;
     }
-    if (len >= 0 && we >= 0.0f && W[hi] > we) W[hi] = we;
+    if (len >= 0 && we >= 0.0f) vr_clamp_end(W[hi], we);
 }
 // Forward sweep of a pure brake profile (tph.calc_vel_profile_brake, mode 'decel_forw': -tyre + drag from wcap on): the
 // step of vr_forward for a brake lane without everything a brake lane does not use (curvature cap, acceleration phases,
@@ -223,9 +276,9 @@ __device__ __noinline__ void vr_brake(const VRCfg c, bool on, const float* __res
         k_prev = kq;
         if (GG) ax_prev = AX[p];
     }
-    if (len >= 0 && we >= 0.0f && W[hi] > we) W[hi] = we;
+    if (len >= 0 && we >= 0.0f) vr_clamp_end(W[hi], we);
 }
-// Backward sweep (flipped arrays, mode 'decel_backw', one look-ahead correction); returns w[lo] afterwards.
+// Backward sweep (VRSweep::bwd on flipped arrays); returns w[lo] afterwards.
 // GG (location dependent local_gg): tph flips radii, el_lengths and the profile for this sweep but NOT the per-point ggv
 // (oracle/tph_port.py:463-538: p_ggv[i] is indexed with the flipped counter), so the point p of the profile [lo, hi] takes
 // the tyre limits of its mirror point lo + hi - p -- reproduced here: K'(p) = |kappa(p)| / ay(mirror), ax(mirror).
@@ -236,33 +289,15 @@ __device__ __noinline__ float vr_backward(const VRCfg c, bool on, const float* _
                                           float wmax) {
     float cur = 0.0f;
     if (on && hi >= lo) {
-        cur = W[hi];
         const int mir = lo + hi;
-        float o_prev = cur;
-        float k_p = GG ? K[hi] * vr_rcp(IAY[hi]) * IAY[mir - hi] : K[hi];
-        float ax_p = GG ? AX[mir - hi] : c.ax_max;
-        bool prev_rise = false, active = false;
+        VRSweep s;
+        s.start(W[hi], GG ? K[hi] * vr_rcp(IAY[hi]) * IAY[mir - hi] : K[hi], GG ? AX[mir - hi] : c.ax_max);
 #pragma unroll 2
         for (int p = hi - 1; p >= lo; --p) {
-            const float o_n = W[p], e2 = E2[p];
             const float kq = GG ? K[p] * vr_rcp(IAY[p]) * IAY[mir - p] : K[p];
-            const float axq = GG ? AX[mir - p] : c.ax_max;
-            const bool rise = o_n > o_prev;
-            active = active || (rise && !prev_rise);
-            const float a = fmaf(cur, c.dm, vr_tire<EXP1>(c, cur, k_p, ax_p));
-            float wn = fmaf(a, e2, cur);
-            const float a2 = fmaf(wn, c.dm, vr_tire<EXP1>(c, wn, kq, axq));
-            const float wt = fmaf(a2, e2, cur);
-            wn = fminf(wn, wt);
-            const float nxt = active ? fminf(wn, o_n) : o_n;
-            active = active && !(wn > wmax);
-            W[p] = nxt;
-            cur = nxt;
-            prev_rise = rise;
-            o_prev = o_n;
-            k_p = kq;
-            ax_p = axq;
+            W[p] = s.bwd<EXP1>(c, W[p], kq, GG ? AX[mir - p] : c.ax_max, E2[p], wmax);
         }
+        cur = s.cur;
     }
     return cur;
 }
@@ -544,8 +579,7 @@ k_vel_res(const LatDev lt, const LtplParams prm, const LtplDims dm, const LtplBu
                     opp_stop_dist += e4[u];
                     ++id;
                     if (id <= ng - 1) {
-                        const double a = acc_brake(ww, k4[u], 14.0, 1.0 / 14.0, prm.dyn_model_exp, dmq);
-                        const double nx = fma(2.0 * a, e4[u], ww);
+                        const double nx = brake_step(ww, k4[u], 14.0, 1.0 / 14.0, prm.dyn_model_exp, dmq, e4[u]);
                         ww = (nx < 0.0) ? 0.0 : nx;
                     } else {
                         ww = 0.0;

@@ -3,8 +3,8 @@
 //
 // Throughput regime (100 k paths x 500 points): one LANE per path, one warp = 32 paths, the path arrays stream through
 // shared memory in tiles of VD_H points x 32 paths (cp.async, transposing on the fly so that a lane reads its path down a
-// conflict-free column).  The recurrences are the fp32 steps of ltpl_vel_res.cuh (w = v^2, branch-free, machine-table
-// segment cached in registers with a warp-uniform miss path).
+// conflict-free column).  Every point takes the fp32 sweep steps of k_vel_res (VRSweep::fwd / bwd with the machine-table
+// segment cache VRSeg, ltpl_vel_res.cuh); this kernel only adds the tiling.
 //   sweep 1 (forward):  kappa, el tiles in -> w tile -> fp32 scratch inside the caller's `ax` rows (4 bytes per point)
 //   sweep 2 (backward): kappa, el, w tiles in -> final w; vx = sqrt(w) and ax = (w1 - w0) / (2 el) leave through the tiles
 // HBM traffic per point: 2 x 16 B in (kappa, el: twice) + 4 B out + 4 B in (w) + 16 B out (vx, ax) = 56 B
@@ -99,10 +99,10 @@ k_velprofile(const __grid_constant__ LtplParams prm, const __grid_constant__ Ltp
     const int ntile = (n + VD_H - 1) / VD_H;
 
     // ---- forward sweep (tph.__solver_fb_acc_profile(backwards=False)) ----
-    float cur = 0.0f, o_prev = 0.0f, k_prev = 0.0f, e_prev = 0.0f;
-    bool prev_rise = false, active = false;
-    int sg = 1;
-    float xlo = c.xl[1], xhi = c.xl[2], x0 = c.x0[1], f0 = c.f0[1], sl = c.sl[1];
+    VRSweep f;   // starts at p = 0
+    VRSeg seg;
+    seg.load(c, 1);
+    float e_prev = 0.0f;
     for (int tl = 0; tl < ntile; ++tl) {
         const int p0 = tl * VD_H;
         vd_load(t_k, vb.kappa, path0, vb.n_paths, n, p0, lane);
@@ -115,39 +115,17 @@ k_velprofile(const __grid_constant__ LtplParams prm, const __grid_constant__ Ltp
             const bool in = p < n;   // warp uniform
             const float kq = (float)(fabs(t_k[k * VD_W + lane]) * inv_ay);
             const float e2 = (float)(2.0 * t_e[k * VD_W + lane]);
-            const float o_n = fminf(vr_rcp(kq), wmax);
-            float nxt;
+            float w;
             if (p == 0) {
-                nxt = fminf(o_n, wcap);
+                w = vr_w_start(kq, wmax, wcap);
+                f.start(w, kq, c.ax_max);
             } else {
-                const bool rise = o_n > o_prev;
-                active = active || (rise && !prev_rise);
-                const float v = vr_sqrt(fmaxf(cur, 0.0f));
-                const bool need = live && in && active;
-                bool miss = need && !(v >= xlo && v < xhi);
-                while (__any_sync(LTPL_FULL, miss)) {
-                    if (miss) sg += (v >= xhi) ? 1 : -1;
-                    xlo = c.xl[sg];
-                    xhi = c.xl[sg + 1];
-                    x0 = c.x0[sg];
-                    f0 = c.f0[sg];
-                    sl = c.sl[sg];
-                    miss = need && !(v >= xlo && v < xhi);
-                }
-                const float a_t = vr_tire<EXP1>(c, cur, k_prev, c.ax_max);
-                const float a = fmaf(-cur, c.dm, fminf(a_t, fmaf(sl, v - x0, f0)));
-                const float wn = fmaf(a, e_prev, cur);
-                nxt = active ? fminf(wn, o_n) : o_n;
-                active = active && !(wn > wmax);
-                prev_rise = rise;
+                // points behind the path end (last tile) step on without storing; nothing reads their state
+                w = f.fwd<EXP1>(c, seg, kq, c.ax_max, e_prev, wmax, live && in);
             }
-            if (in) {
-                o_prev = (p == 0) ? nxt : o_n;
-                cur = nxt;
-                k_prev = kq;
-                e_prev = e2;
-                t_w[k * VD_W + lane] = (p == n - 1 && nxt > we) ? we : nxt;   // v[-1] = min(v[-1], v_end)
-            }
+            e_prev = e2;
+            if (p == n - 1) vr_clamp_end(w, we);
+            if (in) t_w[k * VD_W + lane] = w;
         }
         __syncwarp();
         vd_store_w(t_w, wscr, path0, vb.n_paths, n, p0, lane);
@@ -155,9 +133,8 @@ k_velprofile(const __grid_constant__ LtplParams prm, const __grid_constant__ Ltp
     }
 
     // ---- backward sweep (flipped arrays, mode 'decel_backw', one look-ahead correction); vx, ax on the way ----
-    float k_p = 0.0f, w_next = 0.0f;
-    prev_rise = false;
-    active = false;
+    VRSweep b;   // starts at p = n - 1
+    float w_next = 0.0f;
     for (int tl = ntile - 1; tl >= 0; --tl) {
         const int p0 = tl * VD_H;
         vd_load(t_k, vb.kappa, path0, vb.n_paths, n, p0, lane);
@@ -174,22 +151,13 @@ k_velprofile(const __grid_constant__ LtplParams prm, const __grid_constant__ Ltp
                 const float o_n = t_w[k * VD_W + lane];
                 float wv = o_n, a_out = 0.0f;
                 if (p < n - 1) {
-                    const bool rise = o_n > o_prev;
-                    active = active || (rise && !prev_rise);
-                    const float a = fmaf(cur, c.dm, vr_tire<EXP1>(c, cur, k_p, c.ax_max));
-                    float wn = fmaf(a, e2, cur);
-                    const float a2 = fmaf(wn, c.dm, vr_tire<EXP1>(c, wn, kq, c.ax_max));
-                    wn = fminf(wn, fmaf(a2, e2, cur));
-                    wv = active ? fminf(wn, o_n) : o_n;
-                    active = active && !(wn > wmax);
-                    prev_rise = rise;
+                    wv = b.bwd<EXP1>(c, o_n, kq, c.ax_max, e2, wmax);
                     a_out = (w_next - wv) * vr_rcp(e2);
+                } else {
+                    b.start(o_n, kq, c.ax_max);
                 }
                 t_v[k * VD_W + lane] = (double)vr_sqrt(wv);
                 t_a[k * VD_W + lane] = (double)a_out;
-                cur = wv;
-                o_prev = o_n;
-                k_p = kq;
                 w_next = wv;
             }
         }
