@@ -98,6 +98,19 @@ def check_gg_map(ax, ay, x0, y0, cell):
     return nx, ny, 1.0 / cell
 
 
+def check_gg_planes(ax, ay, batch: int, p_max: int, device) -> None:
+    """input checks of friction planes given as device tensors (BatchPlanner.set_local_gg_planes, the local_gg of a
+    split capture): ``ax``, ``ay`` float64 tensors on ``device`` of equal shape [NSLOT][batch][P <= p_max], any strides.
+    Shapes, dtypes and devices only (no values, no synchronisation); raises ValueError."""
+    for name, a in (("ax", ax), ("ay", ay)):
+        if not isinstance(a, torch.Tensor) or a.device != device or a.dtype != torch.float64:
+            raise ValueError("local_gg planes: %s must be a float64 tensor on %s, got %s" % (
+                name, device, "%s on %s" % (a.dtype, a.device) if isinstance(a, torch.Tensor) else type(a).__name__))
+    if ax.shape != ay.shape or ax.dim() != 3 or tuple(ax.shape[:2]) != (NSLOT, batch) or ax.shape[2] > p_max:
+        raise ValueError("local_gg planes must have the shape [NSLOT][B][P <= p_max] = [%d][%d][<= %d], got %s and %s"
+                         % (NSLOT, batch, p_max, tuple(ax.shape), tuple(ay.shape)))
+
+
 DEFAULT_ONLINE = dict(max_heading_offset=0.8, nmbr_export_points=115, v_max_offset=0.1, max_solutions=1,
                       filt_window_width=1, w_last_edges=[0.0, 0.5, 0.8], controller_type="PD",
                       control_params={"c_p": 1.25, "k_d": 0.025, "k_p": 0.2}, delaycomp=0.1)
@@ -110,6 +123,7 @@ class TickState:
     in_cur: int = 0                  # the device input copy in use (stateful ticks alternate the two)
     pos_last: torch.Tensor = None    # `pos` of the input copy the last tick used: buffers.pos_last of a stateful tick
     gg_planes_used: bool = False     # the last velocity call ran with gg planes (decides the next tick's prev_gg)
+    gg_uploaded: bool = False        # the planes set_local_gg_planes bound last came from host arrays
     zone_key_kept: bool = False      # a staging since allocate(): the next stateful tick applies the zone rule
     zone_key_zero: bool = True       # the device zone keys (_zone_key) are all zero
     zones: tuple = None              # the zone list whose bitmasks are on the device (None: none yet)
@@ -169,6 +183,8 @@ class BatchPlanner(object):
         self.on_device_start = None   # optional callable, called where a stateful tick's host staging ends (timing)
         self._tick = TickState()
         self._generation = 0          # bumped by every change a captured TickGraph cannot follow (tick_graph.py)
+        self._plane_bumps = 0         # the part of _generation set_local_gg_planes bumped (split graphs with planes)
+        self._split_pending = None    # (SplitTickGraph, velocity half) after its replay_paths(), until the next call
         self._traj_base = None        # [1] int32 device id counter of buffers.traj_base, from the first capture on
         self._copy_stream = None      # second stream of plan_stream (trajectory downloads), created on first use
         self.set_vel_params()
@@ -368,25 +384,48 @@ class BatchPlanner(object):
         ``ax``, ``ay`` [NSLOT][B][P] (P <= p_max) = longitudinal / lateral limit at every point of every path (slot 0:
         straight | follow, 1: left, 2: right), aligned with the paths of the last calc_paths; None: back to the constant
         tuple of set_vel_params().  The values are taken without gg_scale (VPFB:213-214 applies it).  Clears the friction
-        map of set_gg_map()."""
+        map of set_gg_map().
+        ``ax``, ``ay`` may also be float64 tensors on the planner's device (any strides, e.g. a friction model evaluated
+        on the device along device_results()["path"]): they are copied into this tick's planes on the current stream,
+        without a host synchronisation, and give the bytes of the same values as NumPy arrays.  Such tensors are
+        checked (device, dtype, shape) before anything changes; a refusal raises ValueError."""
+        on_device = isinstance(ax, torch.Tensor) or isinstance(ay, torch.Tensor)
+        if on_device:
+            check_gg_planes(ax, ay, self.dims.batch, self.dims.p_max, self.device)
         if self._gg_map is not None:   # captured graphs evaluate the map: they go stale with it
             self._generation += 1
         self._gg_map = None
         self.buf.gg_map = None
         if ax is None:
             self._generation += 1
+            self._plane_bumps += 1
+            self._split_pending = None
             self.buf.gg = None
             return
-        ax = np.asarray(ax, dtype=np.float64)
-        ay = np.asarray(ay, dtype=np.float64)
         B, P = self.dims.batch, self.dims.p_max
-        if ax.shape != ay.shape or ax.ndim != 3 or ax.shape[:2] != (NSLOT, B) or ax.shape[2] > P:
-            raise ValueError("local_gg planes must have the shape [NSLOT][B][P <= p_max]")
+        if not on_device:
+            ax = np.asarray(ax, dtype=np.float64)
+            ay = np.asarray(ay, dtype=np.float64)
+            if ax.shape != ay.shape or ax.ndim != 3 or ax.shape[:2] != (NSLOT, B) or ax.shape[2] > P:
+                raise ValueError("local_gg planes must have the shape [NSLOT][B][P <= p_max]")
         self._generation += 1
+        self._plane_bumps += 1
+        self._split_pending = None
+        self._tick.gg_uploaded = not on_device
+        planes = self._gg_planes(self.t)
+        if on_device:   # the given values, then 1.0 behind them: what the host path writes
+            n = ax.shape[2]
+            rows = planes.view(2, NSLOT, B, P)
+            rows[0, :, :, :n].copy_(ax)
+            rows[1, :, :, :n].copy_(ay)
+            if n < P:
+                rows[:, :, :, n:].fill_(1.0)
+            self.buf.gg = planes.data_ptr()
+            return
         host = np.ones((2, NSLOT * B, P))
         host[0, :, :ax.shape[2]] = ax.reshape(NSLOT * B, -1)
         host[1, :, :ay.shape[2]] = ay.reshape(NSLOT * B, -1)
-        self.buf.gg = self._gg_planes(self.t).copy_(torch.from_numpy(host)).data_ptr()
+        self.buf.gg = planes.copy_(torch.from_numpy(host)).data_ptr()
 
     def set_gg_map(self, ax=None, ay=None, x0: float = 0.0, y0: float = 0.0, cell: float = 1.0) -> None:
         """location dependent friction from a map of the track surface, for the whole batch: ``ax``, ``ay`` [ny][nx] =
@@ -469,6 +508,7 @@ class BatchPlanner(object):
         ``tick_args`` = (sel_action, t_const, restart) of a stateful tick: they are staged along, and the tick's zone
         rule applies (a zone under a NEW id is a new zone object: its unblock window is evaluated at this tick,
         OLI:155-237, GLNT:43-77)."""
+        self._split_pending = None
         self._grow_for(sc)
         self._stage_zones(sc.zones)
         ts = self._tick
@@ -646,6 +686,7 @@ class BatchPlanner(object):
                 if a.device != self.t[name].device or a.dtype != torch.float64 or a.numel() != self.t[name].numel():
                     raise ValueError("%s: a float64 tensor of %d values on %s, got %s %s on %s" % (
                         name, self.t[name].numel(), self.t[name].device, a.dtype, tuple(a.shape), a.device))
+        self._split_pending = None
         for name, a in (("pos", pos_est), ("vel_est", vel_est)):
             if isinstance(a, torch.Tensor):
                 self.t[name].copy_(a.reshape(self.t[name].shape))
@@ -758,6 +799,7 @@ class BatchPlanner(object):
 
     # -- kernels ---------------------------------------------------------------------------------------------------------------
     def _call(self, name):
+        self._split_pending = None   # a split replay's velocity half follows only its own paths half
         capi.check(self.lib, getattr(self.lib, name)(self.handle, C.byref(self.params), C.byref(self.dims),
                                                      C.byref(self.buf), self.stream), name)
 
@@ -916,10 +958,30 @@ class BatchPlanner(object):
         from .tick_graph import capture
         return capture(self, True, sc, vel_est=vel_est, sel_action=sel_action, t_const=t_const, restart=restart)
 
-    def _prepare_capture(self, inputs, stateful: bool) -> None:
+    def capture_split_tick(self, sc, vel_est=None, pos_est=None, local_gg=None):
+        """capture a first tick as two halves and return a SplitTickGraph: ``replay_paths()`` = k_stage + set_startpos +
+        calc_paths of ``sc`` (a DeviceScenarioBatch), ``replay_vel_profile()`` = calc_vel_profile with the estimates
+        ``pos_est`` [B][2] / ``vel_est`` [B] (set_estimates) and, with ``local_gg=(ax, ay)``, the friction planes
+        [NSLOT][B][P] (set_local_gg_planes), all float64 device tensors.  Between the two replays the caller may read
+        device_results()["path"] and write the velocity half's inputs (``graph.vel_inputs``) on the device: the
+        reference's loop (calc_paths, then local_gg along the new paths, then calc_vel_profile) with no host work.
+        Everything else as capture_tick; ``local_gg`` excludes a friction map (set_gg_map)."""
+        from .tick_graph import capture_split
+        return capture_split(self, False, sc, vel_est=vel_est, pos_est=pos_est, local_gg=local_gg)
+
+    def capture_next_split_tick(self, sc, sel_action, t_const, vel_est=None, restart=None, pos_est=None,
+                                local_gg=None):
+        """capture a stateful tick as its two halves, next_calc_paths(sc, sel_action, t_const, restart=restart) and
+        next_calc_vel_profile(pos_est, vel_est) with the friction planes ``local_gg`` set between them, and return a
+        SplitTickGraph (see capture_split_tick and capture_next_tick)"""
+        from .tick_graph import capture_split
+        return capture_split(self, True, sc, vel_est=vel_est, pos_est=pos_est, local_gg=local_gg,
+                             sel_action=sel_action, t_const=t_const, restart=restart)
+
+    def _prepare_capture(self, inputs, stateful: bool, planes: bool = False) -> None:
         """everything a tick of these inputs could allocate, grow or copy from the host, done before a capture: the
         buffers for the batch, the memory buffers a stateful tick creates on first use, the zone bitmasks, the id
-        counter and the kernels' attributes (ltpl_prepare_batch)"""
+        counter and the kernels' attributes (ltpl_prepare_batch).  planes: the tick's velocity half sets gg planes"""
         sc = inputs.sc
         pos = self.t["pos"] if stateful else None
         self._grow_for(sc)
@@ -928,6 +990,8 @@ class BatchPlanner(object):
             # stateful tick reads the last tick's positions as pos_last from the current copy; the eager tick keeps the
             # old copy for it instead, so the current copy takes its values here
             self.t["pos"].copy_(pos)
+        if planes:
+            self._gg_planes(self.t)
         if stateful:
             if self._state is None:
                 self._alloc_state()
@@ -938,8 +1002,11 @@ class BatchPlanner(object):
             self._traj_base = torch.full((1,), 10 * self._tick_count, dtype=torch.int32, device=self.device)
         self.buf.traj_base = self._traj_base.data_ptr()
         self.params.traj_base_id = 0
+        buf = capi.Buffers.from_buffer_copy(self.buf)
+        if planes:   # the buffers the velocity half will pass
+            buf.gg = self.t["gg"].data_ptr()
         capi.check(self.lib, self.lib.ltpl_prepare_batch(self.handle, C.byref(self.params), C.byref(self.dims),
-                                                         C.byref(self.buf)), "ltpl_prepare_batch")
+                                                         C.byref(buf)), "ltpl_prepare_batch")
 
     def _host_state(self) -> dict:
         """what a tick changes on the host: the pointer fields and dims a call passes, the buffer dicts (by reference)
@@ -976,9 +1043,14 @@ class BatchPlanner(object):
         [n_export][7] float32 (path (s, b) in row traj_row[s, b]).  For a caller that computes the next tick's
         sel_action / pos_est on the device.  Work queued on the planner's stream after the tick sees them complete.
         The views are valid until the next tick: it rewrites these buffers, and a stateful tick swaps planes by pointer,
-        so read or clone what is needed before staging the next tick."""
+        so read or clone what is needed before staging the next tick.
+        ``path`` [5][NSLOT * B][p_max] float64 holds the planned paths (x, y, psi, kappa, el; row q = slot * B + b,
+        points [0, path_len[slot, b])), valid right after calc_paths / next_calc_paths: a friction model on the device
+        evaluates them for set_local_gg_planes.  A stateful tick swaps this plane by pointer, so the view belongs to
+        the tick that produced it; take device_results() anew after every calc_paths."""
         out = {n: self.t[n] for n in self.DEVICE_RESULTS}
         out["traj"] = self._traj_buf()
+        out["path"] = self.t["path"]
         return out
 
     # -- result access (device -> host, test / facade use) ----------------------------------------------------------------------

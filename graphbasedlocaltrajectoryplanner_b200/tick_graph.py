@@ -1,15 +1,17 @@
 """
 TickGraph -- a first or stateful tick of BatchPlanner captured into CUDA graphs and replayed with no per-tick host work
-(DESIGN.md section 11).  Created by BatchPlanner.capture_tick / capture_next_tick.
+(DESIGN.md section 11).  Created by BatchPlanner.capture_tick / capture_next_tick.  SplitTickGraph -- the same for a
+tick split into its two halves (capture_split_tick / capture_next_split_tick): the paths half, then the velocity half
+with the estimates and friction planes the caller computed on the device in between.
 
 A captured tick keeps the pointers and values it was captured with.  What changes between ticks is handled as follows:
-  - the inputs: the graph reads static device tensors it owns (``graph.inputs``); the caller writes each tick's values
-    into them in place;
+  - the inputs: the graph reads static device tensors it owns (``graph.inputs``, ``paths_inputs`` / ``vel_inputs``);
+    the caller writes each tick's values into them in place;
   - the trajectory ids: they come from a device counter (buffers.traj_base, k_traj_base) instead of the per-call
     params.traj_base_id;
-  - the ping-pong memory of a stateful tick: one graph per state of the planner's buffers (two parities, a third when
-    the first captured tick is also the first with friction planes); a replay runs the graph of the current state and
-    then puts the planner's host side where that tick leaves it, which costs no launch.
+  - the ping-pong memory of a stateful tick: one graph (per half) per state of the planner's buffers (two parities, a
+    third when the first captured tick is also the first with friction planes); a replay runs the graph of the current
+    state and then puts the planner's host side where that tick (half) leaves it, which costs no launch.
 """
 
 from __future__ import annotations
@@ -18,6 +20,7 @@ from dataclasses import dataclass, replace
 
 import torch
 
+from .planner import check_gg_planes
 from .scenarios import DeviceScenarioBatch
 
 _FIELDS = tuple(name for name, _, _ in DeviceScenarioBatch._SPEC)
@@ -40,6 +43,19 @@ def _static(a):
     if any(st == 0 and n > 1 for st, n in zip(a.stride(), a.shape)):
         return a.clone(memory_format=torch.contiguous_format)
     return torch.empty_strided(a.shape, a.stride(), dtype=a.dtype, device=a.device).copy_(a)
+
+
+def _copy_in(what: str, pairs) -> None:
+    """(name, static tensor or None, given value) triples: every captured tensor is required, with its shape and
+    dtype, and nothing else (ValueError before anything is copied); then the copies, on the current stream"""
+    for name, dst, src in pairs:
+        if (dst is None) != (src is None):
+            raise ValueError("%s: %s %s" % (what, name, "was not captured" if dst is None else "is required"))
+        if dst is not None and (not isinstance(src, torch.Tensor) or src.shape != dst.shape or src.dtype != dst.dtype):
+            raise ValueError("%s: %s must be a tensor %s of %s" % (what, name, tuple(dst.shape), dst.dtype))
+    for _, dst, src in pairs:
+        if dst is not None:
+            dst.copy_(src, non_blocking=True)
 
 
 @dataclass
@@ -65,54 +81,73 @@ class TickInputs:
         elif t_const is not None and (self.t_const is None or float(t_const) != self.t_const):
             raise ValueError("TickInputs.copy_: t_const %s" % ("was not captured" if self.t_const is None else
                                                                "was captured as the value %r" % self.t_const))
-        for name, dst, src in pairs:
-            if (dst is None) != (src is None):
-                raise ValueError("TickInputs.copy_: %s %s" % (name, "was not captured" if dst is None else "is required"))
-            if dst is not None and (not isinstance(src, torch.Tensor) or src.shape != dst.shape or src.dtype != dst.dtype):
-                raise ValueError("TickInputs.copy_: %s must be a tensor %s of %s" % (name, tuple(dst.shape), dst.dtype))
-        for _, dst, src in pairs:
-            if dst is not None:
-                dst.copy_(src, non_blocking=True)
+        _copy_in("TickInputs.copy_", pairs)
 
 
-class TickGraph(object):
-    """A tick captured into CUDA graphs (BatchPlanner.capture_tick / capture_next_tick).  ``inputs`` (TickInputs) are
-    the static device inputs; ``replay()`` enqueues the tick on the current stream.  After a replay the planner's
-    results, memory and state are those of the same tick run eagerly.  The graph goes stale when the planner changes
-    in a way it cannot follow (allocate, set_vel_params, set_gg_map, set_local_gg_planes, set_subbatches, grown input
-    buffers): replay() then raises ValueError; capture a new graph.  ``close()`` releases the graphs."""
+@dataclass
+class VelInputs:
+    """the static device inputs of a SplitTickGraph's velocity half: ``pos_est`` [B][2], ``vel_est`` [B] and the
+    friction planes ``ax``, ``ay`` [NSLOT][B][P], float64; None where the capture had none.  Write them in place
+    between replay_paths() and replay_vel_profile(), with copy_() or with device code of your own."""
+    pos_est: torch.Tensor = None
+    vel_est: torch.Tensor = None
+    ax: torch.Tensor = None
+    ay: torch.Tensor = None
 
-    def __init__(self, planner, stateful: bool, inputs: TickInputs, entries: dict, pool, generation: int):
+    def copy_(self, pos_est=None, vel_est=None, local_gg=None) -> None:
+        """the velocity half's values into the static tensors, on the current stream, with the rule of
+        TickInputs.copy_: everything captured is required, nothing else is accepted.  ``local_gg`` = (ax, ay)."""
+        if local_gg is not None and (not isinstance(local_gg, (tuple, list)) or len(local_gg) != 2):
+            raise ValueError("VelInputs.copy_: local_gg must be the pair (ax, ay)")
+        ax, ay = (None, None) if local_gg is None else local_gg
+        _copy_in("VelInputs.copy_", [("pos_est", self.pos_est, pos_est), ("vel_est", self.vel_est, vel_est),
+                                     ("local_gg[0]", self.ax, ax), ("local_gg[1]", self.ay, ay)])
+
+
+class _CapturedTick(object):
+    """what TickGraph and SplitTickGraph share: per state of the planner's buffers one (CUDA graph, host state after
+    it) for each half of the tick, the staleness checks and the release of the graphs"""
+
+    def __init__(self, planner, stateful: bool, entries: dict, pool, own_planes: bool = False):
         self.planner = planner
         self.stateful = stateful
-        self.inputs = inputs
-        self._entries = entries        # planner._tick_key -> (CUDAGraph, host state after the tick)
+        self._entries = entries        # planner._tick_key -> ((CUDAGraph, host state after the half), ...)
         self._pool = pool
-        self._generation = generation
+        self._own_planes = own_planes  # the velocity half sets its planes: set_local_gg_planes does not make it stale
+        self._generation = self._planner_generation()
 
     @property
     def n_graphs(self) -> int:
-        return 0 if self._entries is None else len(self._entries)
+        return 0 if self._entries is None else sum(len(halves) for halves in self._entries.values())
 
-    def replay(self) -> None:
-        """one tick from the current graph inputs, on the current stream: a graph launch plus the host side of the tick
-        (pointer swaps, tick count); no host synchronisation, no host memory read by the device, no library call.
-        Refused with ValueError, changing nothing, on a closed or stale graph, or when the planner's buffers are in a
-        state no graph was captured in."""
+    def _planner_generation(self) -> int:
         pl = self.planner
+        return pl._generation - (pl._plane_bumps if self._own_planes else 0)
+
+    def _check(self, what: str) -> None:
         if self._entries is None:
-            raise ValueError("TickGraph.replay: the graph was closed")
-        if pl._generation != self._generation:
-            raise ValueError("TickGraph.replay: the planner changed since the capture (allocate, set_vel_params, "
-                             "set_gg_map, set_local_gg_planes, set_subbatches or grown input buffers); capture anew")
-        entry = self._entries.get(pl._tick_key(self.stateful))
-        if entry is None:
-            raise ValueError("TickGraph.replay: the planner's buffers are in a state this graph was not captured in "
-                             "(a first-tick graph replays until the next stateful tick); capture anew")
-        graph, after = entry
+            raise ValueError("%s: the graph was closed" % what)
+        if self._planner_generation() != self._generation:
+            raise ValueError("%s: the planner changed since the capture (allocate, set_vel_params, set_gg_map, "
+                             "set_local_gg_planes, set_subbatches or grown input buffers); capture anew" % what)
+
+    def _halves(self, what: str) -> tuple:
+        """the graphs of the planner's current buffer state (ValueError on a closed or stale graph, or a state no
+        graph was captured in)"""
+        self._check(what)
+        halves = self._entries.get(self.planner._tick_key(self.stateful))
+        if halves is None:
+            raise ValueError("%s: the planner's buffers are in a state this graph was not captured in (a first-tick "
+                             "graph replays until the next stateful tick); capture anew" % what)
+        return halves
+
+    def _run(self, half, ends_tick: bool) -> None:
+        graph, after = half
         graph.replay()
+        pl = self.planner
         pl._set_host_state(after)
-        pl._tick_count += 1
+        if ends_tick:
+            pl._tick_count += 1
 
     def close(self) -> None:
         """release the graphs and their memory pool, after waiting for the device (a replay may still run).  Call it
@@ -124,7 +159,7 @@ class TickGraph(object):
         if entries:
             if wait:
                 torch.cuda.synchronize(self.planner.device)
-            _DEFERRED.extend(graph for graph, _ in entries.values())
+            _DEFERRED.extend(graph for halves in entries.values() for graph, _ in halves)
         _release_deferred()
 
     def __del__(self):
@@ -136,14 +171,69 @@ class TickGraph(object):
             pass
 
 
-def capture(pl, stateful: bool, sc, vel_est=None, sel_action=None, t_const=None, restart=None) -> TickGraph:
-    """BatchPlanner.capture_tick (stateful False) / capture_next_tick (True): refusals, static inputs, preparation,
-    then one capture per state of the planner's buffers until the states repeat; the planner's host side is left as
-    it was found"""
-    what = "capture_next_tick" if stateful else "capture_tick"
+class TickGraph(_CapturedTick):
+    """A tick captured into CUDA graphs (BatchPlanner.capture_tick / capture_next_tick).  ``inputs`` (TickInputs) are
+    the static device inputs; ``replay()`` enqueues the tick on the current stream.  After a replay the planner's
+    results, memory and state are those of the same tick run eagerly.  The graph goes stale when the planner changes
+    in a way it cannot follow (allocate, set_vel_params, set_gg_map, set_local_gg_planes, set_subbatches, grown input
+    buffers): replay() then raises ValueError; capture a new graph.  ``close()`` releases the graphs."""
+
+    def __init__(self, planner, stateful: bool, inputs: TickInputs, entries: dict, pool):
+        super().__init__(planner, stateful, entries, pool)
+        self.inputs = inputs
+
+    def replay(self) -> None:
+        """one tick from the current graph inputs, on the current stream: a graph launch plus the host side of the tick
+        (pointer swaps, tick count); no host synchronisation, no host memory read by the device, no library call.
+        Refused with ValueError, changing nothing, on a closed or stale graph, or when the planner's buffers are in a
+        state no graph was captured in."""
+        (half,) = self._halves("TickGraph.replay")
+        self.planner._split_pending = None
+        self._run(half, ends_tick=True)
+
+
+class SplitTickGraph(_CapturedTick):
+    """A tick captured as its two halves (BatchPlanner.capture_split_tick / capture_next_split_tick).  ``paths_inputs``
+    (TickInputs) feed the paths half, ``vel_inputs`` (VelInputs) the velocity half.  ``replay_paths()`` enqueues the
+    paths half; the caller may then read device_results()["path"] and write ``vel_inputs`` with device code of its
+    own; ``replay_vel_profile()`` enqueues the velocity half.  Results, memory and ids are those of the same split
+    calls run eagerly.  The velocity half is refused unless the planner's last call was this graph's replay_paths(),
+    and a replay_paths() is refused while one waits for its velocity half.  Staleness and close() as TickGraph; a
+    graph with friction planes sets them itself, so set_local_gg_planes does not make it stale."""
+
+    def __init__(self, planner, stateful: bool, paths_inputs: TickInputs, vel_inputs: VelInputs, entries: dict, pool):
+        super().__init__(planner, stateful, entries, pool, own_planes=vel_inputs.ax is not None)
+        self.paths_inputs = paths_inputs
+        self.vel_inputs = vel_inputs
+
+    def replay_paths(self) -> None:
+        """the paths half from ``paths_inputs``, on the current stream, with no host work.  Refused with ValueError,
+        changing nothing, like TickGraph.replay, and while an earlier replay_paths() waits for its velocity half."""
+        what = "SplitTickGraph.replay_paths"
+        if self.planner._split_pending is not None:
+            raise ValueError("%s: the last replay_paths() has not had its velocity half (replay_vel_profile())" % what)
+        paths, vel = self._halves(what)
+        self._run(paths, ends_tick=False)
+        self.planner._split_pending = (self, vel)
+
+    def replay_vel_profile(self) -> None:
+        """the velocity half from ``vel_inputs``, on the current stream, with no host work.  Refused with ValueError,
+        changing nothing, unless the planner's last call was this graph's replay_paths(), and on a closed or stale
+        graph."""
+        what = "SplitTickGraph.replay_vel_profile"
+        pending = self.planner._split_pending
+        if pending is None or pending[0] is not self:
+            raise ValueError("%s: the planner's last call was not this graph's replay_paths()" % what)
+        self._check(what)
+        self.planner._split_pending = None
+        self._run(pending[1], ends_tick=True)
+
+
+def _tick_inputs(pl, what: str, stateful: bool, sc, vel_est, sel_action, t_const, restart) -> TickInputs:
+    """the refusals of every capture, then the static inputs of the tick's staging"""
     if not isinstance(sc, DeviceScenarioBatch):
         raise ValueError("%s: needs a DeviceScenarioBatch (a host ScenarioBatch is copied on the host every tick)" % what)
-    if pl._gg_map is None and pl.buf is not None and pl.buf.gg is not None:
+    if pl._gg_map is None and pl.buf is not None and pl.buf.gg is not None and pl._tick.gg_uploaded:
         raise ValueError("%s: uploaded local_gg planes (set_local_gg_planes) are per-tick host data; a friction map "
                          "(set_gg_map) is evaluated inside the tick" % what)
     if stateful:
@@ -154,8 +244,43 @@ def capture(pl, stateful: bool, sc, vel_est=None, sel_action=None, t_const=None,
         if sel_action is None or t_const is None:
             raise ValueError("%s: sel_action and t_const are required" % what)
     vel_est, sel_action, t_const, restart = pl._device_args(sc, vel_est, sel_action, t_const, restart)
-    inputs = TickInputs(replace(sc, **{n: _static(getattr(sc, n)) for n in _FIELDS}), _static(sel_action),
-                        _static(t_const), _static(vel_est), _static(restart))
+    return TickInputs(replace(sc, **{n: _static(getattr(sc, n)) for n in _FIELDS}), _static(sel_action),
+                      _static(t_const), _static(vel_est), _static(restart))
+
+
+def _capture(pl, what: str, stateful: bool, halves) -> tuple:
+    """one CUDA graph per half (callables) per state of the planner's buffers, from the current state until the
+    states repeat; the planner's host side, tick count and generation are left as they were found.  Returns the
+    entries and the memory pool."""
+    _release_deferred()
+    pool = torch.cuda.graph_pool_handle()
+    side = torch.cuda.Stream(device=pl.device)
+    before = (pl._host_state(), pl._tick_count, pl._generation, pl._plane_bumps, pl._split_pending)
+    entries = {}
+    try:
+        key = pl._tick_key(stateful)
+        while key not in entries:
+            if len(entries) == 3:
+                raise RuntimeError("%s: the planner's buffers did not return to a captured state" % what)
+            graphs = []
+            for run in halves:
+                graph = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(graph, pool=pool, stream=side):
+                    run()
+                graphs.append((graph, pl._host_state()))
+            entries[key] = tuple(graphs)
+            key = pl._tick_key(stateful)
+    finally:
+        pl._set_host_state(before[0])
+        pl._tick_count, pl._generation, pl._plane_bumps, pl._split_pending = before[1:]
+    return entries, pool
+
+
+def capture(pl, stateful: bool, sc, vel_est=None, sel_action=None, t_const=None, restart=None) -> TickGraph:
+    """BatchPlanner.capture_tick (stateful False) / capture_next_tick (True): refusals, static inputs, preparation,
+    then one capture per state of the planner's buffers until the states repeat"""
+    what = "capture_next_tick" if stateful else "capture_tick"
+    inputs = _tick_inputs(pl, what, stateful, sc, vel_est, sel_action, t_const, restart)
     pl._prepare_capture(inputs, stateful)
 
     def run():
@@ -166,22 +291,49 @@ def capture(pl, stateful: bool, sc, vel_est=None, sel_action=None, t_const=None,
             pl.set_startpos()
             pl.tick()
 
-    _release_deferred()
-    pool = torch.cuda.graph_pool_handle()
-    side = torch.cuda.Stream(device=pl.device)
-    before, tick_count = pl._host_state(), pl._tick_count
-    entries = {}
-    try:
-        key = pl._tick_key(stateful)
-        while key not in entries:
-            if len(entries) == 3:
-                raise RuntimeError("%s: the planner's buffers did not return to a captured state" % what)
-            graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph, pool=pool, stream=side):
-                run()
-            entries[key] = (graph, pl._host_state())
-            key = pl._tick_key(stateful)
-    finally:
-        pl._set_host_state(before)
-        pl._tick_count = tick_count
-    return TickGraph(pl, stateful, inputs, entries, pool, pl._generation)
+    entries, pool = _capture(pl, what, stateful, [run])
+    return TickGraph(pl, stateful, inputs, entries, pool)
+
+
+def capture_split(pl, stateful: bool, sc, vel_est=None, pos_est=None, local_gg=None, sel_action=None, t_const=None,
+                  restart=None) -> SplitTickGraph:
+    """BatchPlanner.capture_split_tick (stateful False) / capture_next_split_tick (True): the refusals of capture()
+    and those of the velocity half's inputs, static inputs, preparation, then the halves of every buffer state"""
+    what = "capture_next_split_tick" if stateful else "capture_split_tick"
+    if isinstance(sc, DeviceScenarioBatch):
+        B = sc.size
+        if pos_est is not None and (not isinstance(pos_est, torch.Tensor) or pos_est.device != pl.device
+                                    or pos_est.dtype != torch.float64 or tuple(pos_est.shape) != (B, 2)):
+            raise ValueError("%s: pos_est must be a float64 tensor [%d][2] on %s" % (what, B, pl.device))
+        if local_gg is not None:
+            if pl._gg_map is not None:
+                raise ValueError("%s: local_gg planes and a friction map (set_gg_map) exclude each other" % what)
+            if not isinstance(local_gg, (tuple, list)) or len(local_gg) != 2:
+                raise ValueError("%s: local_gg must be the pair (ax, ay)" % what)
+            check_gg_planes(local_gg[0], local_gg[1], B, pl.cap["p_max"], pl.device)
+    inputs = _tick_inputs(pl, what, stateful, sc, None, sel_action, t_const, restart)
+    vel_est = pl._device_args(sc, vel_est)[0]
+    ax, ay = (None, None) if local_gg is None else local_gg
+    vel_inputs = VelInputs(*(_static(a) for a in (pos_est, vel_est, ax, ay)))
+    pl._prepare_capture(inputs, stateful, planes=local_gg is not None)
+
+    def paths():
+        if stateful:
+            pl.next_calc_paths(inputs.sc, inputs.sel_action, inputs.t_const, restart=inputs.restart)
+        else:
+            pl.stage_scenarios(inputs.sc)
+            pl.set_startpos()
+            pl.calc_paths()
+
+    def vel():
+        if vel_inputs.ax is not None:
+            pl.set_local_gg_planes(vel_inputs.ax, vel_inputs.ay)
+        if stateful:
+            pl.next_calc_vel_profile(pos_est=vel_inputs.pos_est, vel_est=vel_inputs.vel_est)
+        else:
+            if vel_inputs.pos_est is not None or vel_inputs.vel_est is not None:
+                pl.set_estimates(vel_inputs.pos_est, vel_inputs.vel_est)
+            pl.calc_vel_profile()
+
+    entries, pool = _capture(pl, what, stateful, [paths, vel])
+    return SplitTickGraph(pl, stateful, inputs, vel_inputs, entries, pool)
