@@ -36,7 +36,7 @@ import numpy as np
 
 from . import capi
 from .lattice import load_or_build_lattice
-from .planner import BatchPlanner, read_online_config
+from .planner import BatchPlanner, check_prefer, read_online_config
 from .scenarios import ScenarioBatch
 
 # required path dict entries (LTPL:22-23)
@@ -326,20 +326,33 @@ class Graph_LTPL(object):
         pl.calc_vel_profile()
         return pl.download()
 
-    def plan_batch(self, scenarios=None, synchronize: bool = True) -> dict:
+    def plan_batch(self, scenarios=None, synchronize: bool = True, prefer=None) -> dict:
         """One end-to-end batched tick: host scenario arrays -> (H2D) -> set_startpos -> calc_paths -> calc_vel_profile
         -> (D2H) -> pinned host action sets: ``traj`` [n_rows][n_export][7] fp32 (compact: one row per kept
         trajectory), ``exp_q`` (row -> path id q = slot * B + b), ``traj_row`` [NSLOT][B] (path -> row or -1),
         ``traj_len``, ``traj_id``, ``action_id``, ``status``, ``sc_flags``, ``n_rows``.
         With ``scenarios=None`` the previously staged batch is planned again.  A DeviceScenarioBatch skips the host
-        staging and the H2D copy (BatchPlanner.stage_scenarios); the results are downloaded all the same."""
+        staging and the H2D copy (BatchPlanner.stage_scenarios); the results are downloaded all the same.
+        With ``prefer`` (BatchPlanner.select: a list of action names, or ids [B][L]) one trajectory per scenario is
+        selected on the device and BatchPlanner.download_selected()'s result replaces the compact rows: ``sel_info``
+        [B][4] (action, row, rows, id), ``sel_action`` [B] and ``sel_traj`` [B][n_export][7], scenario b in row b.
+        A bad ``prefer`` raises ValueError before anything is staged or launched."""
         pl = self.planner
+        if prefer is not None:
+            batch = scenarios.size if scenarios is not None else (pl.dims.batch if pl.dims is not None else None)
+            if batch is None:
+                raise ValueError("plan_batch: prefer without a staged batch")
+            check_prefer(prefer, batch, pl.device)
         if scenarios is not None:
             pl.stage_scenarios(scenarios)
         pl.upload()
         pl.set_startpos()
         pl.tick()
-        out = pl.download()
+        if prefer is not None:
+            pl.select(prefer)
+            out = pl.download_selected()
+        else:
+            out = pl.download()
         if synchronize:
             import torch
             torch.cuda.current_stream(pl.device).synchronize()
@@ -353,8 +366,8 @@ class Graph_LTPL(object):
         indexed or iterated; the arrays are views of the pinned host buffer (fp32), nothing is copied."""
         return ActionSetView(out)
 
-    def plan_stream(self, batches, vel_est=None, device_hook=None):
+    def plan_stream(self, batches, vel_est=None, device_hook=None, prefer=None):
         """Pipelined variant of ``plan_batch`` over an iterable of ScenarioBatch objects: yields one result dict per
         batch, in order; the device-to-host copy of step i overlaps the kernels of step i + 1
-        (``BatchPlanner.plan_stream``)."""
-        return self.planner.plan_stream(batches, vel_est=vel_est, device_hook=device_hook)
+        (``BatchPlanner.plan_stream``).  ``prefer``: as plan_batch, every step selects and downloads the selection."""
+        return self.planner.plan_stream(batches, vel_est=vel_est, device_hook=device_hook, prefer=prefer)

@@ -18,8 +18,9 @@ NSLOT = 3
 MAX_AXM = 32
 
 ACT_NONE, ACT_STRAIGHT, ACT_FOLLOW, ACT_LEFT, ACT_RIGHT = -1, 0, 1, 2, 3
-ACT_EMERGENCY = 4   # only as the executed action of a stateful tick (OTH:307-309)
+ACT_EMERGENCY = 4   # only as the executed action of a stateful tick (OTH:307-309) and in preference lists (select)
 ACTION_NAMES = {ACT_STRAIGHT: "straight", ACT_FOLLOW: "follow", ACT_LEFT: "left", ACT_RIGHT: "right"}
+SELECT_MAX = 8      # entries of a preference list (LtplSelect.prefer_len)
 
 ST_FOUND, ST_REDUCED_HORIZON, ST_TIE_AMBIGUOUS, ST_START_BLOCKED = 1, 2, 4, 8
 ST_TRAJ_VALID, ST_VEL_BOUND_VIOL, ST_TOO_CLOSE, ST_CONST_ONLY, ST_RENAMED_STRAIGHT = 16, 32, 64, 128, 256
@@ -107,11 +108,22 @@ class StageSrc(C.Structure):
                 ("sel_action_bytes", C.c_int32), ("restart_bytes", C.c_int32), ("zone_key_rule", C.c_int32)]
 
 
+class Select(C.Structure):
+    """LtplSelect; it carries its size (struct_bytes), which ltpl_select_batch checks at every call"""
+    _fields_ = [("struct_bytes", C.c_int32), ("prefer_len", C.c_int32), ("prefer", C.c_void_p),
+                ("prefer_s", C.c_int64 * 2), ("prefer_bytes", C.c_int32), ("sel_action", C.c_void_p),
+                ("sel_action_s", C.c_int64), ("sel_info", C.c_void_p), ("sel_traj", C.c_void_p)]
+
+    def __init__(self):
+        super().__init__()
+        self.struct_bytes = C.sizeof(Select)
+
+
 EXPORTS = ("ltpl_version", "ltpl_last_error", "ltpl_sizeof", "ltpl_max_objects", "ltpl_lattice_create",
            "ltpl_lattice_destroy", "ltpl_set_startpos_batch", "ltpl_calc_paths_batch", "ltpl_calc_vel_profile_batch",
            "ltpl_tick_batch", "ltpl_velprofile_batch", "ltpl_launch_count", "ltpl_launch_stage", "ltpl_next_tick_batch",
            "ltpl_next_calc_paths_batch", "ltpl_next_calc_vel_profile_batch", "ltpl_set_subbatches",
-           "ltpl_stage_inputs_batch", "ltpl_prepare_batch")
+           "ltpl_stage_inputs_batch", "ltpl_prepare_batch", "ltpl_select_batch")
 
 
 def build_library(verbose: bool = False) -> str:
@@ -171,6 +183,9 @@ def load_library():
     lib.ltpl_stage_inputs_batch.restype = C.c_int
     lib.ltpl_prepare_batch.argtypes = [C.c_void_p, C.POINTER(Params), C.POINTER(Dims), C.POINTER(Buffers)]
     lib.ltpl_prepare_batch.restype = C.c_int
+    lib.ltpl_select_batch.argtypes = [C.POINTER(Params), C.POINTER(Dims), C.POINTER(Buffers), C.POINTER(Select),
+                                      C.c_void_p]
+    lib.ltpl_select_batch.restype = C.c_int
     if lib.ltpl_version() != ABI_VERSION:
         raise RuntimeError("libltpl_b200.so ABI version %d != binding %d" % (lib.ltpl_version(), ABI_VERSION))
     for which, st in enumerate((LatticeHeader, Params, Dims, Buffers, VelBatch, StageSrc)):

@@ -23,6 +23,7 @@
 #include "ltpl_gg_map.cuh"
 #include "ltpl_stage.cuh"
 #include "ltpl_traj_base.cuh"
+#include "ltpl_select.cuh"
 
 // the memory records are the int32 arrays BatchPlanner allocates: st_info [B][8], trim [NSLOT*B][4]
 static_assert(sizeof(LtplStateInfo) == 8 * sizeof(int32_t) && alignof(LtplStateInfo) == alignof(int32_t), "st_info row");
@@ -680,6 +681,27 @@ int ltpl_stage_inputs_batch(const LtplDims* dm, const LtplBuffers* bf, const Ltp
         return fail("stage: src.zone_key_rule needs src.zone_key_last and buffers.zone_s0");
     k_stage<<<ctas(dm->batch), kThreads, 0, static_cast<cudaStream_t>(stream)>>>(*dm, *bf, *src);
     return check_launch("k_stage");
+}
+
+int ltpl_select_batch(const LtplParams* prm, const LtplDims* dm, const LtplBuffers* bf, const LtplSelect* sel,
+                      void* stream) {
+    if (!prm || !dm || !bf || !sel) return fail("null argument");
+    if (sel->struct_bytes != (int32_t)sizeof(LtplSelect))
+        return fail("select: sel.struct_bytes must be sizeof(LtplSelect) (the caller's layout of the struct differs)");
+    if (dm->batch <= 0 || dm->n_export < 1) return fail("dims.batch and dims.n_export must be > 0");
+    if (!bf->action_id || !bf->traj_row || !bf->traj_len || !bf->traj_id)
+        return fail("select: buffers action_id, traj_row, traj_len and traj_id must be set");
+    if (prm->incl_emerg_traj && !bf->em_info) return fail("select: params.incl_emerg_traj needs buffers.em_info");
+    if (!sel->sel_action) return fail("select: sel.sel_action must be set");
+    if (!sel->sel_info) return fail("select: sel.sel_info must be set");
+    if (sel->prefer_len < 0 || sel->prefer_len > LTPL_SELECT_MAX)
+        return fail("select: sel.prefer_len must be in [0, LTPL_SELECT_MAX = 8]");
+    if (sel->prefer_len > 0 && !sel->prefer) return fail("select: sel.prefer must be set when sel.prefer_len > 0");
+    if (sel->prefer_bytes != 1 && sel->prefer_bytes != 4 && sel->prefer_bytes != 8)
+        return fail("select: sel.prefer_bytes must be 1, 4 or 8");
+    if (sel->sel_traj && !bf->traj) return fail("select: sel.sel_traj needs buffers.traj");
+    k_select<<<ctas(dm->batch), kThreads, 0, static_cast<cudaStream_t>(stream)>>>(*dm, *bf, *sel, prm->incl_emerg_traj);
+    return check_launch("k_select");
 }
 
 #ifdef LTPL_PROFILE_PHASES

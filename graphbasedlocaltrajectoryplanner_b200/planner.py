@@ -111,6 +111,40 @@ def check_gg_planes(ax, ay, batch: int, p_max: int, device) -> None:
                          % (NSLOT, batch, p_max, tuple(ax.shape), tuple(ay.shape)))
 
 
+PREFER_IDS = {"straight": capi.ACT_STRAIGHT, "follow": capi.ACT_FOLLOW, "left": capi.ACT_LEFT, "right": capi.ACT_RIGHT,
+              "emergency": capi.ACT_EMERGENCY}
+_PREFER_DTYPES = (torch.int8, torch.uint8, torch.int32, torch.int64)
+
+
+def check_prefer(prefer, batch: int, device):
+    """input checks of an action preference (BatchPlanner.select): a list of action names (PREFER_IDS; one list for the
+    whole batch), a host integer array [batch][L] or an integer tensor [batch][L] on ``device`` (int8, uint8, int32 or
+    int64, any strides), L <= capi.SELECT_MAX.  Names, shapes, dtypes and devices only (no tensor values, no
+    synchronisation); raises ValueError.  Returns the tensor as it is, or the ids as an int64 NumPy array [1][L] (a
+    list) or [batch][L] (an array)."""
+    if isinstance(prefer, torch.Tensor):
+        if prefer.device != torch.device(device) or prefer.dtype not in _PREFER_DTYPES:
+            raise ValueError("prefer: a tensor must be int8 / uint8 / int32 / int64 on %s, got %s on %s"
+                             % (device, prefer.dtype, prefer.device))
+        ids = prefer
+    elif isinstance(prefer, (list, tuple)):
+        bad = [a for a in prefer if not isinstance(a, str) or a not in PREFER_IDS]
+        if bad:
+            raise ValueError("prefer: unknown action name(s) %s; the names are %s" % (bad, sorted(PREFER_IDS)))
+        ids = np.array([[PREFER_IDS[a] for a in prefer]], dtype=np.int64).reshape(1, len(prefer))
+    elif isinstance(prefer, np.ndarray):
+        if prefer.dtype.kind not in "iu":
+            raise ValueError("prefer: a host array must hold integers, got %s" % prefer.dtype)
+        ids = prefer.astype(np.int64)
+    else:
+        raise ValueError("prefer: a list of action names, an integer array or a device tensor [B][L], got %s"
+                         % type(prefer).__name__)
+    rows = 1 if isinstance(prefer, (list, tuple)) else batch
+    if ids.ndim != 2 or ids.shape[0] != rows or ids.shape[1] > capi.SELECT_MAX:
+        raise ValueError("prefer: shape [%d][L <= %d], got %s" % (batch, capi.SELECT_MAX, tuple(ids.shape)))
+    return ids
+
+
 DEFAULT_ONLINE = dict(max_heading_offset=0.8, nmbr_export_points=115, v_max_offset=0.1, max_solutions=1,
                       filt_window_width=1, w_last_edges=[0.0, 0.5, 0.8], controller_type="PD",
                       control_params={"c_p": 1.25, "k_d": 0.025, "k_p": 0.2}, delaycomp=0.1)
@@ -129,6 +163,8 @@ class TickState:
     zones: tuple = None              # the zone list whose bitmasks are on the device (None: none yet)
     staged_on_device: bool = False   # the last staged batch was a DeviceScenarioBatch: upload() has nothing to copy
     ticked: bool = False             # the buffers hold a tick (a velocity call ran since they were allocated)
+    emerg: bool = False              # the last velocity call ran with incl_emerg_traj ('emergency' for select)
+    selected: bool = False           # select() ran since the last velocity call: sel_action="selected" may be staged
 
 
 class BatchPlanner(object):
@@ -187,6 +223,7 @@ class BatchPlanner(object):
         self._split_pending = None    # (SplitTickGraph, velocity half) after its replay_paths(), until the next call
         self._traj_base = None        # [1] int32 device id counter of buffers.traj_base, from the first capture on
         self._copy_stream = None      # second stream of plan_stream (trajectory downloads), created on first use
+        self._sel = self._sel_host = None   # per set: selection buffers of select(), device / pinned (created on use)
         self.set_vel_params()
 
     def __del__(self):
@@ -364,6 +401,7 @@ class BatchPlanner(object):
         self._state = None   # buffers of the stateful tick, allocated by next_tick()
         # further compact export buffers: the pipelined stream planner lets the D2H of step i overlap step i + 1
         self.traj_bufs = [t["traj"]] + [z(((NSLOT + 1) * B, NE, 7), f32) for _ in range(self.N_SETS - 1)]
+        self._sel, self._sel_host = [None] * self.N_SETS, [None] * self.N_SETS
         # pinned host staging of the per-tick results (N_SETS sets for the pipelined path)
         pin = lambda shape, dt: torch.zeros(shape, dtype=dt).pin_memory()   # noqa: E731
         self.h_meta_raw, self.h_out_sets = [], []
@@ -730,14 +768,17 @@ class BatchPlanner(object):
         """the compact export buffer of traj_bufs that buffers.traj points at (the one the last tick wrote)"""
         return next(tb for tb in self.traj_bufs if tb.data_ptr() == self.buf.traj)
 
-    def plan_stream(self, batches, vel_est=None, device_hook=None):
+    def plan_stream(self, batches, vel_est=None, device_hook=None, prefer=None):
         """Pipelined end-to-end planning of a sequence of ScenarioBatch objects (generator of result dicts, in order).
 
         Per step: host staging (pinned) -> H2D -> k_startpos -> tick kernels -> D2H of the per-path arrays on the compute
         stream; the large D2H of the compact trajectory rows runs on a second stream and overlaps the kernels of the
         next step (CUDA events for the hand-over).  With N_SETS = 3 staging / export buffer sets the host stages step
         i + 1 while the GPU runs step i and the copy engine drains step i - 1, so the GPU never waits for the host.
-        Results are views of pinned host memory; a result stays valid until N_SETS - 1 further results were taken."""
+        Results are views of pinned host memory; a result stays valid until N_SETS - 1 further results were taken.
+        With ``prefer`` (see select) every step selects one trajectory per scenario on the device and its result is
+        download_selected()'s dict instead: the fixed-size copy of the selected rows is issued on the second stream
+        without waiting for the row count."""
         ns = self.N_SETS
         compute = torch.cuda.current_stream(self.device)
         if self._copy_stream is None:
@@ -749,6 +790,15 @@ class BatchPlanner(object):
         inflight = []         # sets whose trajectory copy is issued, oldest first
 
         def issue_copy(k):
+            if prefer is not None:   # fixed size: the copy stream waits for the step on the device, not the host
+                copy_stream.wait_event(ev_meta[k])
+                with torch.cuda.stream(copy_stream):
+                    results[k] = self._copy_selected(k)
+                    ev = torch.cuda.Event()
+                    ev.record(copy_stream)
+                ev_d2h[k] = ev
+                inflight.append(k)
+                return
             ev_meta[k].synchronize()
             out = self.h_out_sets[k]
             n = int(out["queue_cnt"][2])
@@ -760,8 +810,10 @@ class BatchPlanner(object):
             ev_d2h[k] = ev
             out["n_rows"] = n
             out["incl_emerg_traj"] = bool(self.params.incl_emerg_traj)
+            results[k] = out
             inflight.append(k)
 
+        results = [None] * ns   # per set: the dict a step yields
         try:
             for i, sc in enumerate(batches):
                 k = i % ns
@@ -771,10 +823,12 @@ class BatchPlanner(object):
                     # hand out finished results in order; the set about to be reused must have left the device first
                     j = inflight.pop(0)
                     ev_d2h[j].synchronize()
-                    yield self.h_out_sets[j]
+                    yield results[j]
                 if isinstance(sc, DeviceScenarioBatch):
                     raise ValueError("plan_stream overlaps the host staging of ScenarioBatch objects; plan a "
                                      "DeviceScenarioBatch with plan_batch or tick()")
+                if prefer is not None and i == 0:
+                    prefer = self._prefer_tensor(check_prefer(prefer, sc.size, self.device))
                 if device_hook is not None and hasattr(device_hook, "before"):
                     device_hook.before(k)   # e.g. wait until a collective that still reads buffer set k has finished
                 self.stage_scenarios(sc, vel_est=vel_est, which=k)
@@ -782,6 +836,8 @@ class BatchPlanner(object):
                 self.upload(which=k)
                 self.set_startpos()
                 self.tick()
+                if prefer is not None:
+                    self._select(prefer, None, k)
                 if device_hook is not None:     # e.g. an all-gather of the device-side action sets (multi-GPU)
                     device_hook(k)
                 self._download_meta(k)
@@ -793,15 +849,106 @@ class BatchPlanner(object):
                 issue_copy(pending.pop(0))
             for j in inflight:
                 ev_d2h[j].synchronize()
-                yield self.h_out_sets[j]
+                yield results[j]
         finally:
-            self.buf.traj = self.traj_bufs[0].data_ptr()
+            if self.buf is not None:   # (a refusal may come before the first batch allocated anything)
+                self.buf.traj = self.traj_bufs[0].data_ptr()
 
     # -- kernels ---------------------------------------------------------------------------------------------------------------
     def _call(self, name):
         self._split_pending = None   # a split replay's velocity half follows only its own paths half
         capi.check(self.lib, getattr(self.lib, name)(self.handle, C.byref(self.params), C.byref(self.dims),
                                                      C.byref(self.buf), self.stream), name)
+
+    # -- the trajectory each scenario takes (ltpl_select_batch, csrc/ltpl_select.cuh) ---------------------------------------
+    def select(self, prefer, sel_action=None) -> dict:
+        """the reference loop's step after every tick, on the device: per scenario the first action of ``prefer`` that
+        the last velocity call returned (main_min_example.py:83-85) -- a slot action whose trajectory was kept, or
+        'emergency' when that call had incl_emerg_traj and kept anything (OTH:1027-1034).
+        ``prefer``: a list of action names (PREFER_IDS) for the whole batch, a host integer array [B][L] or an integer
+        tensor [B][L] on the planner's device (any strides) of action ids (capi.ACT_*; other values are skipped),
+        L <= capi.SELECT_MAX.  Enqueues one kernel on the current stream, without a host synchronisation, and returns
+        device views the planner owns, valid until the next select(): ``sel_action`` [B] int32 (capi.ACT_NONE where
+        nothing in the list was returned), ``sel_info`` [B][4] int32 (action, row in device_results()["traj"] or -1,
+        rows, trajectory id) and ``sel_traj`` [B][n_export][7] float32 (a copy of the selected row, zeros without a
+        selection).  ``sel_action``: an int32 tensor [B] on the device (any stride) that receives the actions instead.
+        The next stateful tick takes these actions with sel_action="selected".  Bad arguments raise ValueError before
+        anything is launched."""
+        self._check_select("select")
+        prefer = check_prefer(prefer, self.dims.batch, self.device)
+        if sel_action is not None and (not isinstance(sel_action, torch.Tensor) or sel_action.device != self.device
+                                       or sel_action.dtype != torch.int32 or tuple(sel_action.shape) != (self.dims.batch,)):
+            raise ValueError("select: sel_action must be an int32 tensor [%d] on %s" % (self.dims.batch, self.device))
+        return self._select(self._prefer_tensor(prefer), sel_action, 0)
+
+    def _check_select(self, what: str) -> None:
+        if self.buf is None or not self._tick.ticked:
+            raise ValueError("%s: no velocity call ran on this planner's buffers" % what)
+        if all(tb.data_ptr() != self.buf.traj for tb in self.traj_bufs):
+            raise ValueError("%s: buffers.traj points at peer memory (a PeerGather is attached)" % what)
+
+    def _sel_buffers(self, which: int) -> dict:
+        """the device selection buffers of set ``which``, created on first use for the allocated batch: ``info`` [B][4]
+        int32, ``traj`` [B][n_export][7] float32"""
+        if self._sel[which] is None:
+            B, NE = self.dims.batch, self.dims.n_export
+            self._sel[which] = dict(info=torch.full((B, 4), -1, dtype=torch.int32, device=self.device),
+                                    traj=torch.zeros((B, NE, 7), dtype=torch.float32, device=self.device))
+        return self._sel[which]
+
+    def _prefer_tensor(self, prefer) -> torch.Tensor:
+        """a preference checked by check_prefer as a device tensor: host ids are copied from pinned memory on the current
+        stream, without a host synchronisation"""
+        if isinstance(prefer, torch.Tensor):
+            return prefer
+        return torch.from_numpy(prefer).pin_memory().to(self.device, non_blocking=True)
+
+    def _select(self, prefer: torch.Tensor, sel_action, which: int) -> dict:
+        """k_select into selection set ``which`` (sel_action None: column 0 of its info)"""
+        sel = self._sel_buffers(which)
+        out = sel["info"][:, 0] if sel_action is None else sel_action
+        s = capi.Select()
+        s.prefer_len = int(prefer.shape[1])
+        s.prefer_bytes = prefer.element_size()
+        if s.prefer_len:
+            s.prefer = prefer.data_ptr()
+            s.prefer_s[0] = 0 if prefer.shape[0] == 1 else prefer.stride(0)   # one list for the batch
+            s.prefer_s[1] = prefer.stride(1)
+        s.sel_action, s.sel_action_s = out.data_ptr(), out.stride(0)
+        s.sel_info, s.sel_traj = sel["info"].data_ptr(), sel["traj"].data_ptr()
+        prm = capi.Params.from_buffer_copy(self.params)
+        prm.incl_emerg_traj = int(self._tick.emerg)
+        capi.check(self.lib, self.lib.ltpl_select_batch(C.byref(prm), C.byref(self.dims), C.byref(self.buf), C.byref(s),
+                                                        self.stream), "ltpl_select_batch")
+        self._tick.selected = True
+        return dict(sel_action=out, sel_info=sel["info"], sel_traj=sel["traj"])
+
+    def download_selected(self, which: int = 0) -> dict:
+        """the last tick's small per-path arrays (as download()) and the selection of the last select(): ``sel_info``
+        [B][4], ``sel_action`` (its column 0) and ``sel_traj`` [B][n_export][7], copied into pinned host memory on the
+        current stream, both copies back to back, then one synchronisation.  The rows have a fixed size (scenario b in
+        row b), so nothing is read back first.  Views of pinned buffers, valid until the next download_selected()."""
+        if self._sel is None or self._sel[0] is None:
+            raise ValueError("download_selected: no select() ran on this planner's buffers")
+        self._download_meta(which)
+        out = self._copy_selected(which, 0)
+        torch.cuda.current_stream(self.device).synchronize()
+        return out
+
+    def _copy_selected(self, which: int, sel_set: int = None) -> dict:
+        """the D2H copy of selection set ``sel_set`` (default: ``which``) into its pinned buffers on the current stream,
+        and the result dict with the per-path arrays of host set ``which`` (_download_meta)"""
+        sel_set = which if sel_set is None else sel_set
+        if self._sel_host[sel_set] is None:
+            self._sel_host[sel_set] = {k: torch.empty(v.shape, dtype=v.dtype, pin_memory=True)
+                                       for k, v in self._sel[sel_set].items()}
+        h = self._sel_host[sel_set]
+        for k in ("info", "traj"):
+            h[k].copy_(self._sel[sel_set][k], non_blocking=True)
+        out = {n: self.h_out_sets[which][n] for n in self._meta_names}
+        out.update(sel_info=h["info"], sel_action=h["info"][:, 0], sel_traj=h["traj"],
+                   incl_emerg_traj=bool(self._tick.emerg))
+        return out
 
     def _call_vel(self, name):
         """a call that includes calc_vel_profile: its trajectories get the next ids (+10 per call, OTH:669).  Once a
@@ -812,6 +959,7 @@ class BatchPlanner(object):
         self._call(name)
         self._tick.gg_planes_used = self.buf.gg is not None
         self._tick.ticked = True
+        self._tick.emerg, self._tick.selected = bool(self.params.incl_emerg_traj), False
 
     def set_startpos(self) -> None:
         self._call("ltpl_set_startpos_batch")
@@ -871,6 +1019,9 @@ class BatchPlanner(object):
         # before the swaps below: refused inputs change nothing
         if sel_action is None or t_const is None:
             raise ValueError("stateful tick: sel_action and t_const are required")
+        selected = self._selected(sel_action) if isinstance(sel_action, str) else None
+        if selected is not None:   # a device batch stages the selection through k_stage, a host batch copies it below
+            sel_action = selected if isinstance(sc, DeviceScenarioBatch) else 0
         if isinstance(sc, DeviceScenarioBatch):
             vel_est, sel_action, t_const, restart = self._device_args(sc, vel_est, sel_action, t_const, restart)
         else:
@@ -908,6 +1059,17 @@ class BatchPlanner(object):
         buf.restart = None if restart is None else st["restart"].data_ptr()
         self._stage(sc, vel_est, 0, (sel_action, t_const, restart))
         self.upload()   # a ScenarioBatch: ONE packed H2D copy (k_stage has written a DeviceScenarioBatch)
+        if selected is not None and not isinstance(sc, DeviceScenarioBatch):
+            t["sel_action"].copy_(selected)
+
+    def _selected(self, name: str) -> torch.Tensor:
+        """sel_action="selected": the actions of the last select() (column 0 of its sel_info, a device view), which must
+        have run after the last velocity call"""
+        if name != "selected":
+            raise ValueError('sel_action: action ids or "selected", got %r' % name)
+        if not self._tick.selected:
+            raise ValueError('sel_action="selected": no select() ran after the last velocity call')
+        return self._sel[0]["info"][:, 0]
 
     def next_calc_paths(self, sc: ScenarioBatch, sel_action, t_const, vel_est=None, restart=None) -> None:
         """calc_paths of a stateful tick (OTH:289-516 with the iterative memory): ``sc`` carries the object
@@ -915,6 +1077,7 @@ class BatchPlanner(object):
         scenario executed since the last tick, ``t_const`` = min(average calculation time * calc_time_safety, 0.5) per
         scenario (OTH:353-375; the caller keeps the moving average).  The previous tick (tick() / calc_paths() +
         calc_vel_profile() after set_startpos(), or a stateful tick) must have run on this planner.
+        ``sel_action="selected"`` takes the actions of the last select() on the device, without a copy through the host.
         ``restart``: boolean array [B]; a true entry restarts that scenario inside this tick, as set_startpos(sc.pos[b],
         sc.heading[b], sc.vel[b]) on a live planner followed by a first tick (its memory is dropped, its sel_action and
         t_const are ignored); the other scenarios keep theirs.  A wrong shape raises ValueError and changes nothing.
@@ -938,50 +1101,57 @@ class BatchPlanner(object):
         self._call_vel("ltpl_next_tick_batch")
 
     # -- ticks replayed from CUDA graphs (tick_graph.py, DESIGN.md section 11) -------------------------------------------
-    def capture_tick(self, sc, vel_est=None, restart=None):
+    def capture_tick(self, sc, vel_est=None, restart=None, prefer=None):
         """capture a first tick -- k_stage + set_startpos + tick of ``sc`` (a DeviceScenarioBatch) -- into a CUDA graph
         and return a TickGraph: write each tick's inputs into ``graph.inputs`` (TickInputs.copy_) and call
         ``graph.replay()``, which enqueues the tick with no host work.  The arguments are those of the eager device
         calls.  Everything that could allocate or copy from the host happens here, before the capture (a batch of
         another size starts a new session, as in stage_scenarios); the zone list ``sc.zones`` is fixed for the graph's
-        lifetime.  Nothing is launched and the planner's state is left as it was."""
+        lifetime.  Nothing is launched and the planner's state is left as it was.
+        ``prefer`` (see select): the graph ends with select(prefer) from a device copy it owns (``graph.prefer``, which
+        may be rewritten in place), so a replay leaves the selection for a stateful tick with sel_action="selected"."""
         from .tick_graph import capture
         if restart is not None:
             raise ValueError("capture_tick: a first tick takes no restart mask (capture_next_tick does)")
-        return capture(self, False, sc, vel_est=vel_est)
+        return capture(self, False, sc, vel_est=vel_est, prefer=prefer)
 
-    def capture_next_tick(self, sc, sel_action, t_const, vel_est=None, restart=None):
+    def capture_next_tick(self, sc, sel_action, t_const, vel_est=None, restart=None, prefer=None):
         """capture a stateful tick (next_tick with the same arguments) into CUDA graphs, one per ping-pong parity of
         the planner's buffers, and return a TickGraph (see capture_tick).  A replay runs the graph of the planner's
         current parity and then does the host side of the tick (pointer swaps, tick count), so eager ticks and replays
-        may be interleaved freely.  Needs a previous tick in this session and the session's batch size."""
+        may be interleaved freely.  Needs a previous tick in this session and the session's batch size.
+        ``sel_action="selected"`` stages the last selection on the device (see next_calc_paths); with ``prefer`` every
+        per-parity graph ends with select(prefer): replays then run a closed loop with no host work for the pick."""
         from .tick_graph import capture
-        return capture(self, True, sc, vel_est=vel_est, sel_action=sel_action, t_const=t_const, restart=restart)
+        return capture(self, True, sc, vel_est=vel_est, sel_action=sel_action, t_const=t_const, restart=restart,
+                       prefer=prefer)
 
-    def capture_split_tick(self, sc, vel_est=None, pos_est=None, local_gg=None):
+    def capture_split_tick(self, sc, vel_est=None, pos_est=None, local_gg=None, prefer=None):
         """capture a first tick as two halves and return a SplitTickGraph: ``replay_paths()`` = k_stage + set_startpos +
         calc_paths of ``sc`` (a DeviceScenarioBatch), ``replay_vel_profile()`` = calc_vel_profile with the estimates
         ``pos_est`` [B][2] / ``vel_est`` [B] (set_estimates) and, with ``local_gg=(ax, ay)``, the friction planes
         [NSLOT][B][P] (set_local_gg_planes), all float64 device tensors.  Between the two replays the caller may read
         device_results()["path"] and write the velocity half's inputs (``graph.vel_inputs``) on the device: the
         reference's loop (calc_paths, then local_gg along the new paths, then calc_vel_profile) with no host work.
-        Everything else as capture_tick; ``local_gg`` excludes a friction map (set_gg_map)."""
+        Everything else as capture_tick; ``local_gg`` excludes a friction map (set_gg_map).  With ``prefer`` the velocity
+        half ends with select(prefer), as in capture_tick."""
         from .tick_graph import capture_split
-        return capture_split(self, False, sc, vel_est=vel_est, pos_est=pos_est, local_gg=local_gg)
+        return capture_split(self, False, sc, vel_est=vel_est, pos_est=pos_est, local_gg=local_gg, prefer=prefer)
 
     def capture_next_split_tick(self, sc, sel_action, t_const, vel_est=None, restart=None, pos_est=None,
-                                local_gg=None):
+                                local_gg=None, prefer=None):
         """capture a stateful tick as its two halves, next_calc_paths(sc, sel_action, t_const, restart=restart) and
         next_calc_vel_profile(pos_est, vel_est) with the friction planes ``local_gg`` set between them, and return a
         SplitTickGraph (see capture_split_tick and capture_next_tick)"""
         from .tick_graph import capture_split
         return capture_split(self, True, sc, vel_est=vel_est, pos_est=pos_est, local_gg=local_gg,
-                             sel_action=sel_action, t_const=t_const, restart=restart)
+                             sel_action=sel_action, t_const=t_const, restart=restart, prefer=prefer)
 
-    def _prepare_capture(self, inputs, stateful: bool, planes: bool = False) -> None:
+    def _prepare_capture(self, inputs, stateful: bool, planes: bool = False, select: bool = False) -> None:
         """everything a tick of these inputs could allocate, grow or copy from the host, done before a capture: the
         buffers for the batch, the memory buffers a stateful tick creates on first use, the zone bitmasks, the id
-        counter and the kernels' attributes (ltpl_prepare_batch).  planes: the tick's velocity half sets gg planes"""
+        counter and the kernels' attributes (ltpl_prepare_batch).  planes: the tick's velocity half sets gg planes;
+        select: the tick ends with select() (its buffers)"""
         sc = inputs.sc
         pos = self.t["pos"] if stateful else None
         self._grow_for(sc)
@@ -992,6 +1162,8 @@ class BatchPlanner(object):
             self.t["pos"].copy_(pos)
         if planes:
             self._gg_planes(self.t)
+        if select:
+            self._sel_buffers(0)
         if stateful:
             if self._state is None:
                 self._alloc_state()

@@ -11,7 +11,9 @@ A captured tick keeps the pointers and values it was captured with.  What change
     params.traj_base_id;
   - the ping-pong memory of a stateful tick: one graph (per half) per state of the planner's buffers (two parities, a
     third when the first captured tick is also the first with friction planes); a replay runs the graph of the current
-    state and then puts the planner's host side where that tick (half) leaves it, which costs no launch.
+    state and then puts the planner's host side where that tick (half) leaves it, which costs no launch;
+  - the executed action (sel_action="selected"): the graph stages the planner's selection buffer, and with ``prefer``
+    the tick (its velocity half) ends with select(), so every replay leaves the selection the next replay stages.
 """
 
 from __future__ import annotations
@@ -20,7 +22,7 @@ from dataclasses import dataclass, replace
 
 import torch
 
-from .planner import check_gg_planes
+from .planner import check_gg_planes, check_prefer
 from .scenarios import DeviceScenarioBatch
 
 _FIELDS = tuple(name for name, _, _ in DeviceScenarioBatch._SPEC)
@@ -62,7 +64,8 @@ def _copy_in(what: str, pairs) -> None:
 class TickInputs:
     """the static device inputs of a TickGraph.  Write each tick's values into them in place before replay() -- with
     copy_() below or with the tensors' own copy_.  ``t_const`` is a tensor [B], or the float the graph was captured
-    with (fixed); ``sc.zones`` is the zone list fixed at capture."""
+    with (fixed); ``sc.zones`` is the zone list fixed at capture.  ``sel_action`` is the name "selected" when the graph
+    stages the planner's selection (nothing to copy)."""
     sc: DeviceScenarioBatch
     sel_action: torch.Tensor = None
     t_const: object = None
@@ -74,8 +77,9 @@ class TickInputs:
         with is required, with its shape and dtype, and nothing else (ValueError before anything is copied).
         ``sc.zones`` is not read."""
         pairs = [("sc." + n, getattr(self.sc, n), getattr(sc, n)) for n in _FIELDS]
-        pairs += [(n, getattr(self, n), a) for n, a in (("sel_action", sel_action), ("vel_est", vel_est),
-                                                        ("restart", restart))]
+        captured_sel = None if isinstance(self.sel_action, str) else self.sel_action
+        pairs += [("sel_action", captured_sel, sel_action)]
+        pairs += [(n, getattr(self, n), a) for n, a in (("vel_est", vel_est), ("restart", restart))]
         if isinstance(self.t_const, torch.Tensor):
             pairs.append(("t_const", self.t_const, t_const))
         elif t_const is not None and (self.t_const is None or float(t_const) != self.t_const):
@@ -178,9 +182,10 @@ class TickGraph(_CapturedTick):
     in a way it cannot follow (allocate, set_vel_params, set_gg_map, set_local_gg_planes, set_subbatches, grown input
     buffers): replay() then raises ValueError; capture a new graph.  ``close()`` releases the graphs."""
 
-    def __init__(self, planner, stateful: bool, inputs: TickInputs, entries: dict, pool):
+    def __init__(self, planner, stateful: bool, inputs: TickInputs, entries: dict, pool, prefer=None):
         super().__init__(planner, stateful, entries, pool)
         self.inputs = inputs
+        self.prefer = prefer   # the device preference the graph's select() reads (None: no select)
 
     def replay(self) -> None:
         """one tick from the current graph inputs, on the current stream: a graph launch plus the host side of the tick
@@ -201,10 +206,12 @@ class SplitTickGraph(_CapturedTick):
     and a replay_paths() is refused while one waits for its velocity half.  Staleness and close() as TickGraph; a
     graph with friction planes sets them itself, so set_local_gg_planes does not make it stale."""
 
-    def __init__(self, planner, stateful: bool, paths_inputs: TickInputs, vel_inputs: VelInputs, entries: dict, pool):
+    def __init__(self, planner, stateful: bool, paths_inputs: TickInputs, vel_inputs: VelInputs, entries: dict, pool,
+                 prefer=None):
         super().__init__(planner, stateful, entries, pool, own_planes=vel_inputs.ax is not None)
         self.paths_inputs = paths_inputs
         self.vel_inputs = vel_inputs
+        self.prefer = prefer   # the device preference the velocity half's select() reads (None: no select)
 
     def replay_paths(self) -> None:
         """the paths half from ``paths_inputs``, on the current stream, with no host work.  Refused with ValueError,
@@ -230,7 +237,8 @@ class SplitTickGraph(_CapturedTick):
 
 
 def _tick_inputs(pl, what: str, stateful: bool, sc, vel_est, sel_action, t_const, restart) -> TickInputs:
-    """the refusals of every capture, then the static inputs of the tick's staging"""
+    """the refusals of every capture, then the static inputs of the tick's staging (sel_action="selected" stays the
+    name: the graph stages the planner's selection buffer)"""
     if not isinstance(sc, DeviceScenarioBatch):
         raise ValueError("%s: needs a DeviceScenarioBatch (a host ScenarioBatch is copied on the host every tick)" % what)
     if pl._gg_map is None and pl.buf is not None and pl.buf.gg is not None and pl._tick.gg_uploaded:
@@ -243,9 +251,34 @@ def _tick_inputs(pl, what: str, stateful: bool, sc, vel_est, sel_action, t_const
             raise ValueError("%s: batch of %d scenarios, the session has %d" % (what, sc.size, pl.dims.batch))
         if sel_action is None or t_const is None:
             raise ValueError("%s: sel_action and t_const are required" % what)
-    vel_est, sel_action, t_const, restart = pl._device_args(sc, vel_est, sel_action, t_const, restart)
-    return TickInputs(replace(sc, **{n: _static(getattr(sc, n)) for n in _FIELDS}), _static(sel_action),
-                      _static(t_const), _static(vel_est), _static(restart))
+    selected = isinstance(sel_action, str)
+    if selected:
+        pl._selected(sel_action)
+    vel_est, sel_action, t_const, restart = pl._device_args(sc, vel_est, None if selected else sel_action, t_const,
+                                                            restart)
+    return TickInputs(replace(sc, **{n: _static(getattr(sc, n)) for n in _FIELDS}),
+                      "selected" if selected else _static(sel_action), _static(t_const), _static(vel_est),
+                      _static(restart))
+
+
+def _check_selected(what: str, sel_action, prefer) -> None:
+    """a graph that stages the selection (sel_action="selected") has to make the next one itself: with prefer"""
+    if isinstance(sel_action, str) and prefer is None:
+        raise ValueError('%s: sel_action="selected" needs prefer, so that every replay leaves the selection the next '
+                         'one stages' % what)
+
+
+def _prefer(pl, what: str, prefer, batch: int):
+    """the graph's own device copy of a preference (check_prefer), made before the capture"""
+    if prefer is None:
+        return None
+    try:
+        ids = check_prefer(prefer, batch, pl.device)
+    except ValueError as e:
+        raise ValueError("%s: %s" % (what, e)) from None
+    if not isinstance(ids, torch.Tensor):
+        ids = torch.as_tensor(ids).to(pl.device)
+    return _static(ids)
 
 
 def _capture(pl, what: str, stateful: bool, halves) -> tuple:
@@ -276,12 +309,14 @@ def _capture(pl, what: str, stateful: bool, halves) -> tuple:
     return entries, pool
 
 
-def capture(pl, stateful: bool, sc, vel_est=None, sel_action=None, t_const=None, restart=None) -> TickGraph:
+def capture(pl, stateful: bool, sc, vel_est=None, sel_action=None, t_const=None, restart=None, prefer=None) -> TickGraph:
     """BatchPlanner.capture_tick (stateful False) / capture_next_tick (True): refusals, static inputs, preparation,
     then one capture per state of the planner's buffers until the states repeat"""
     what = "capture_next_tick" if stateful else "capture_tick"
+    _check_selected(what, sel_action, prefer)
     inputs = _tick_inputs(pl, what, stateful, sc, vel_est, sel_action, t_const, restart)
-    pl._prepare_capture(inputs, stateful)
+    prefer = _prefer(pl, what, prefer, sc.size)
+    pl._prepare_capture(inputs, stateful, select=prefer is not None)
 
     def run():
         if stateful:
@@ -290,16 +325,19 @@ def capture(pl, stateful: bool, sc, vel_est=None, sel_action=None, t_const=None,
             pl.stage_scenarios(inputs.sc, vel_est=inputs.vel_est)
             pl.set_startpos()
             pl.tick()
+        if prefer is not None:
+            pl._select(prefer, None, 0)
 
     entries, pool = _capture(pl, what, stateful, [run])
-    return TickGraph(pl, stateful, inputs, entries, pool)
+    return TickGraph(pl, stateful, inputs, entries, pool, prefer)
 
 
 def capture_split(pl, stateful: bool, sc, vel_est=None, pos_est=None, local_gg=None, sel_action=None, t_const=None,
-                  restart=None) -> SplitTickGraph:
+                  restart=None, prefer=None) -> SplitTickGraph:
     """BatchPlanner.capture_split_tick (stateful False) / capture_next_split_tick (True): the refusals of capture()
     and those of the velocity half's inputs, static inputs, preparation, then the halves of every buffer state"""
     what = "capture_next_split_tick" if stateful else "capture_split_tick"
+    _check_selected(what, sel_action, prefer)
     if isinstance(sc, DeviceScenarioBatch):
         B = sc.size
         if pos_est is not None and (not isinstance(pos_est, torch.Tensor) or pos_est.device != pl.device
@@ -315,7 +353,8 @@ def capture_split(pl, stateful: bool, sc, vel_est=None, pos_est=None, local_gg=N
     vel_est = pl._device_args(sc, vel_est)[0]
     ax, ay = (None, None) if local_gg is None else local_gg
     vel_inputs = VelInputs(*(_static(a) for a in (pos_est, vel_est, ax, ay)))
-    pl._prepare_capture(inputs, stateful, planes=local_gg is not None)
+    prefer = _prefer(pl, what, prefer, sc.size)
+    pl._prepare_capture(inputs, stateful, planes=local_gg is not None, select=prefer is not None)
 
     def paths():
         if stateful:
@@ -334,6 +373,8 @@ def capture_split(pl, stateful: bool, sc, vel_est=None, pos_est=None, local_gg=N
             if vel_inputs.pos_est is not None or vel_inputs.vel_est is not None:
                 pl.set_estimates(vel_inputs.pos_est, vel_inputs.vel_est)
             pl.calc_vel_profile()
+        if prefer is not None:
+            pl._select(prefer, None, 0)
 
     entries, pool = _capture(pl, what, stateful, [paths, vel])
-    return SplitTickGraph(pl, stateful, inputs, vel_inputs, entries, pool)
+    return SplitTickGraph(pl, stateful, inputs, vel_inputs, entries, pool, prefer)

@@ -36,7 +36,8 @@ extern "C" {
 #define LTPL_ACT_FOLLOW 1
 #define LTPL_ACT_LEFT 2
 #define LTPL_ACT_RIGHT 3
-#define LTPL_ACT_EMERGENCY 4 /* only as `sel_action`: the caller executed the 'emergency' trajectory (OTH:307-309) */
+#define LTPL_ACT_EMERGENCY 4 /* only as `sel_action` (the caller executed the 'emergency' trajectory, OTH:307-309) */
+                             /* and in the preference lists of ltpl_select_batch                                    */
 
 /* action slots per scenario: slot 0 = straight | follow (mutually exclusive, MOPG:124-174), 1 = left, 2 = right */
 #define LTPL_NSLOT 3
@@ -366,6 +367,27 @@ typedef struct LtplStageSrc {
     int32_t zone_key_rule;   /* non-zero: a stateful tick, zone_s0[b] = -1 where the key changed and is non-zero        */
 } LtplStageSrc;
 
+/* The trajectory each scenario takes after a velocity call (ltpl_select_batch): the first action of a preference list  */
+/* that the call returned -- the step the reference's loops take after every tick (main_min_example.py:83-85).  A slot   */
+/* action a is returned when some slot s has action_id[s][b] == a and traj_row[s][b] >= 0; 'emergency' when the call ran */
+/* with params.incl_emerg_traj, some slot trajectory was kept and em_info[b][0] >= 0 (OTH:1027-1034).                   */
+/* The struct carries its own size: an addition to the library that leaves every earlier struct as it was, so the ABI  */
+/* version of those stays, and a binding with another idea of this struct is refused at the call.                     */
+#define LTPL_SELECT_MAX 8
+typedef struct LtplSelect {
+    int32_t struct_bytes;    /* sizeof(LtplSelect) as the caller compiled it; anything else is refused                   */
+    int32_t prefer_len;      /* 0 .. LTPL_SELECT_MAX entries per list                                                    */
+    const void* prefer;      int64_t prefer_s[2];  /* [B][prefer_len] action ids LTPL_ACT_*, DEVICE pointer, strides in      */
+                                                   /* elements; prefer_s[0] = 0: one list for the whole batch.  Entries     */
+                                                   /* that are not one of the five ids are skipped                          */
+    int32_t prefer_bytes;    /* 1, 4 or 8: integer size of the list entries                                              */
+    int32_t* sel_action;     int64_t sel_action_s; /* [B] the selected action id or LTPL_ACT_NONE, e.g. straight into the   */
+                                                   /* array LtplStageSrc.sel_action of the next stateful tick reads         */
+    int32_t* sel_info;       /* [B][4] action, row in buffers.traj (-1: none), rows (traj_len / em_info[b][1], 0: none),  */
+                             /*        trajectory id (traj_id / em_info[b][2], -1: none)                                  */
+    float* sel_traj;         /* [B][n_export][7] a copy of the selected row, zeros without a selection; NULL: not copied */
+} LtplSelect;
+
 int ltpl_version(void);
 const char* ltpl_last_error(void);
 int ltpl_sizeof(int which); /* 0 header, 1 params, 2 dims, 3 buffers, 4 velbatch, 5 stage src: ABI self check for the ctypes mirror */
@@ -418,6 +440,13 @@ int ltpl_velprofile_batch(const LtplParams* prm, const LtplVelBatch* vb, void* s
 /* src.restart buf.restart (0 / 1), with src.zone_key_rule the zone rule of a stateful tick (buf.zone_s0).  Values are     */
 /* taken as they are; the tick clamps n_obj, n_pred and zone_sel as it does for host inputs.                             */
 int ltpl_stage_inputs_batch(const LtplDims* dims, const LtplBuffers* buf, const LtplStageSrc* src, void* stream);
+
+/* the selection of every scenario after a velocity call (LtplSelect), in ONE launch on the stream (k_select): reads     */
+/* action_id, traj_row, traj_len, traj_id, em_info and traj as the call left them, so launch it on the call's stream    */
+/* behind it (behind k_traj_base, so a tick replayed from a graph reports the same ids as an eager one).  `prm` is the  */
+/* params of that call (incl_emerg_traj).  No lattice: the selection does not depend on it.                          */
+int ltpl_select_batch(const LtplParams* prm, const LtplDims* dims, const LtplBuffers* buf, const LtplSelect* sel,
+                      void* stream);
 
 /* Sets, for these lattice / params / dims / buffers, every per-kernel attribute a tick entry point would otherwise set   */
 /* on its first launch (dynamic shared-memory limits of k_plan, k_path and the velocity kernel, k_plan's carveout);      */
