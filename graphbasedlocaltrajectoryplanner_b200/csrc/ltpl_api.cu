@@ -651,14 +651,69 @@ int ltpl_launch_stage(int stage, const LtplLattice* lat, const LtplParams* prm, 
 
 int ltpl_velprofile_batch(const LtplParams* prm, const LtplVelBatch* vb, void* stream) {
     if (!prm || !vb) return fail("null argument");
-    if (vb->n_paths <= 0 || vb->n_points < 2) return fail("velprofile: need n_paths > 0 and n_points >= 2");
-    if (prm->n_axm < 1 || prm->n_axm > LTPL_MAX_AXM) return fail("params.n_axm out of range");
-    if (prm->axm_v[prm->n_axm - 1] < prm->vel_max)
-        return fail("ax_max_machines has to cover the entire velocity range of the car (i.e. >= v_max)!");
-    if (prm->dyn_model_exp == 1.0)
-        k_velprofile<true><<<(vb->n_paths + 31) / 32, 32, VD_SMEM_BYTES, static_cast<cudaStream_t>(stream)>>>(*prm, *vb);
-    else
-        k_velprofile<false><<<(vb->n_paths + 31) / 32, 32, VD_SMEM_BYTES, static_cast<cudaStream_t>(stream)>>>(*prm, *vb);
+    LtplVelPlan vp = {};
+    vp.struct_bytes = (int32_t)sizeof(LtplVelPlan);
+    vp.mode = LTPL_VP_PROFILE;
+    vp.n_paths = vb->n_paths;
+    vp.n_points = vb->n_points;
+    vp.kappa = vb->kappa;
+    vp.el = vb->el;
+    vp.v_start = vb->v_start;
+    vp.v_end = vb->v_end;
+    vp.vx = vb->vx;
+    vp.ax = vb->ax;
+    vp.kappa_s = vp.el_s = vp.out_s = vb->n_points;
+    return ltpl_vel_plan_batch(prm, &vp, stream);
+}
+
+int ltpl_vel_plan_batch(const LtplParams* prm, const LtplVelPlan* vp, void* stream) {
+    if (!prm || !vp) return fail("null argument");
+    if (vp->struct_bytes != (int32_t)sizeof(LtplVelPlan))
+        return fail("vel_plan: vp.struct_bytes must be sizeof(LtplVelPlan) (the caller's layout of the struct differs)");
+    const bool brake = vp->mode == LTPL_VP_BRAKE;
+    if (!brake && vp->mode != LTPL_VP_PROFILE) return fail("vel_plan: vp.mode must be LTPL_VP_PROFILE or LTPL_VP_BRAKE");
+    if (vp->n_paths <= 0) return fail("vel_plan: vp.n_paths must be > 0");
+    const int n = vp->n_points;
+    if (n < 2) return fail("vel_plan: vp.n_points must be >= 2");
+    if (!vp->kappa) return fail("vel_plan: vp.kappa must be set");
+    if (!vp->el) return fail("vel_plan: vp.el must be set");
+    if (!vp->v_start) return fail("vel_plan: vp.v_start must be set");
+    if (!brake && !vp->v_end) return fail("vel_plan: vp.v_end must be set (LTPL_VP_PROFILE)");
+    if (!vp->vx) return fail("vel_plan: vp.vx must be set");
+    if (!vp->ax) return fail("vel_plan: vp.ax must be set");
+    if (vp->kappa_s < n) return fail("vel_plan: vp.kappa_s must be >= n_points");
+    if (vp->el_s < n - 1) return fail("vel_plan: vp.el_s must be >= n_points - 1");
+    if (vp->gg && vp->gg_s < 2 * (int64_t)n) return fail("vel_plan: vp.gg_s must be >= 2 n_points");
+    if (vp->out_s < n) return fail("vel_plan: vp.out_s must be >= n_points");
+    if (!brake) {   // the machine limits only bound the profile mode
+        if (prm->n_axm < 1 || prm->n_axm > LTPL_MAX_AXM) return fail("params.n_axm out of range");
+        if (prm->axm_v[prm->n_axm - 1] < prm->vel_max)
+            return fail("ax_max_machines has to cover the entire velocity range of the car (i.e. >= v_max)!");
+    }
+    const LtplVelBatch vb = {vp->n_paths, n, vp->kappa, vp->el, vp->v_start, vp->v_end, vp->vx, vp->ax};
+    VdLayout a;
+    a.n_pts = vp->n_pts;
+    a.gg = vp->gg;
+    a.k_s = vp->kappa_s;
+    a.e_s = vp->el_s;
+    a.g_s = vp->gg_s;
+    a.o_s = vp->out_s;
+    const bool gg = vp->gg != nullptr;
+    const int grid = (vp->n_paths + 31) / 32;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (brake) {
+        (gg ? k_velbrake<true> : k_velbrake<false>)<<<grid, 32, vd_smem_brake(gg), st>>>(*prm, vb, a);
+        return check_launch("k_velbrake");
+    }
+    // the dense constant-friction solver: rows of n_points and one length; anything else takes the general layout
+    const bool ragged = vp->n_pts || vp->kappa_s != n || vp->el_s != n || vp->out_s != n;
+    const int kind = (prm->dyn_model_exp == 1.0 ? 1 : 0) + (gg ? 2 : 0) + (ragged ? 4 : 0);
+    static void (*const kFns[8])(LtplParams, LtplVelBatch, VdLayout) = {
+        k_velprofile<false, false, false>, k_velprofile<true, false, false>, k_velprofile<false, true, false>,
+        k_velprofile<true, true, false>,   k_velprofile<false, false, true>, k_velprofile<true, false, true>,
+        k_velprofile<false, true, true>,   k_velprofile<true, true, true>};
+    const int smem = (gg || ragged) ? vd_smem_general(gg) : VD_SMEM_BYTES;
+    kFns[kind]<<<grid, 32, smem, st>>>(*prm, vb, a);
     return check_launch("k_velprofile");
 }
 

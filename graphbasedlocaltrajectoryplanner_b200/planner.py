@@ -111,6 +111,45 @@ def check_gg_planes(ax, ay, batch: int, p_max: int, device) -> None:
                          % (NSLOT, batch, p_max, tuple(ax.shape), tuple(ay.shape)))
 
 
+def fill_vel_params(p, online: dict, veh: dict, vel_max: float, gg_scale: float, local_gg, ax_max_machines,
+                    safety_d: float, incl_emerg_traj: bool) -> None:
+    """fills LtplParams ``p`` from the online ini keys (``online``, see read_online_config), the vehicle parameters of
+    graph_init (``veh``: dyn_model_exp, drag_coeff, m_veh) and the per-call arguments of Graph_LTPL.calc_vel_profile
+    (LTPL:344-352).  Every check runs before the first field is written: a refused call leaves ``p`` as it was."""
+    if type(local_gg) is not tuple or len(local_gg) != 2:   # OTH:651-653 (dict form: Graph_LTPL / set_local_gg_planes)
+        raise ValueError("Provided local_gg does not satisfy requested format! Read parameter documentation.")
+    axm = np.atleast_2d(np.asarray(ax_max_machines, dtype=np.float64))
+    if axm.shape[1] != 2:
+        raise RuntimeError("ax_max_machines must consist of the two columns [vx, ax_max_machines]!")
+    if axm.shape[0] > capi.MAX_AXM:
+        raise ValueError("ax_max_machines has more than %d rows" % capi.MAX_AXM)
+    if axm[-1, 0] < vel_max:                               # tph.calc_vel_profile input check
+        raise RuntimeError("ax_max_machines has to cover the entire velocity range of the car (i.e. >= v_max)!")
+    o = online
+    if o["controller_type"] not in ("PD", "PDtan"):
+        raise ValueError('Unsupported control type "' + o["controller_type"] + '"!')
+    p.max_heading_offset = o["max_heading_offset"]
+    p.v_max_offset = o["v_max_offset"]
+    cp = o["control_params"]
+    p.follow_c_p, p.follow_k_d, p.follow_k_p = cp["c_p"], cp["k_d"], cp["k_p"]
+    p.follow_tan_w = cp.get("tan_w", 1.0)
+    p.follow_control_type = 0 if o["controller_type"] == "PD" else 1
+    p.nmbr_export_points = int(o["nmbr_export_points"])
+    p.dyn_model_exp, p.drag_coeff, p.m_veh = veh["dyn_model_exp"], veh["drag_coeff"], veh["m_veh"]
+    p.vel_max, p.gg_scale, p.gg_ax, p.gg_ay, p.safety_d = vel_max, gg_scale, local_gg[0], local_gg[1], safety_d
+    p.n_axm = axm.shape[0]
+    p.delaycomp = float(o.get("delaycomp", 0.1))
+    for i in range(3):
+        p.w_last_edges[i] = float(o["w_last_edges"][i]) if i < len(o["w_last_edges"]) else 1.0
+    p.incl_emerg_traj = 1 if incl_emerg_traj else 0
+    p.filt_window = int(o["filt_window_width"])
+    for i in range(axm.shape[0]):
+        p.axm_v[i] = axm[i, 0]
+        p.axm_a[i] = axm[i, 1]
+    for i in range(axm.shape[0] - 1):   # slopes exactly as np.interp forms them
+        p.axm_s[i] = (axm[i + 1, 1] - axm[i, 1]) / (axm[i + 1, 0] - axm[i, 0])
+
+
 PREFER_IDS = {"straight": capi.ACT_STRAIGHT, "follow": capi.ACT_FOLLOW, "left": capi.ACT_LEFT, "right": capi.ACT_RIGHT,
               "emergency": capi.ACT_EMERGENCY}
 _PREFER_DTYPES = (torch.int8, torch.uint8, torch.int32, torch.int64)
@@ -248,40 +287,9 @@ class BatchPlanner(object):
         """per-call arguments of Graph_LTPL.calc_vel_profile (LTPL:344-352)."""
         if local_gg is None:        # location dependent friction: the planes of set_local_gg_planes() are used
             local_gg = (1.0, 1.0)
-        if type(local_gg) is not tuple or len(local_gg) != 2:   # OTH:651-653 (dict form: Graph_LTPL / set_local_gg_planes)
-            raise ValueError("Provided local_gg does not satisfy requested format! Read parameter documentation.")
-        axm = np.atleast_2d(np.asarray(ax_max_machines, dtype=np.float64))
-        if axm.shape[1] != 2:
-            raise RuntimeError("ax_max_machines must consist of the two columns [vx, ax_max_machines]!")
-        if axm.shape[0] > capi.MAX_AXM:
-            raise ValueError("ax_max_machines has more than %d rows" % capi.MAX_AXM)
-        if axm[-1, 0] < vel_max:                               # tph.calc_vel_profile input check
-            raise RuntimeError("ax_max_machines has to cover the entire velocity range of the car (i.e. >= v_max)!")
+        fill_vel_params(self.params, self.online, self.veh, vel_max=vel_max, gg_scale=gg_scale, local_gg=local_gg,
+                        ax_max_machines=ax_max_machines, safety_d=safety_d, incl_emerg_traj=incl_emerg_traj)
         self._generation += 1   # after the checks: a refused call leaves captured graphs valid
-        p = self.params
-        o = self.online
-        p.max_heading_offset = o["max_heading_offset"]
-        p.v_max_offset = o["v_max_offset"]
-        cp = o["control_params"]
-        p.follow_c_p, p.follow_k_d, p.follow_k_p = cp["c_p"], cp["k_d"], cp["k_p"]
-        p.follow_tan_w = cp.get("tan_w", 1.0)
-        if o["controller_type"] not in ("PD", "PDtan"):
-            raise ValueError('Unsupported control type "' + o["controller_type"] + '"!')
-        p.follow_control_type = 0 if o["controller_type"] == "PD" else 1
-        p.nmbr_export_points = int(o["nmbr_export_points"])
-        p.dyn_model_exp, p.drag_coeff, p.m_veh = self.veh["dyn_model_exp"], self.veh["drag_coeff"], self.veh["m_veh"]
-        p.vel_max, p.gg_scale, p.gg_ax, p.gg_ay, p.safety_d = vel_max, gg_scale, local_gg[0], local_gg[1], safety_d
-        p.n_axm = axm.shape[0]
-        p.delaycomp = float(o.get("delaycomp", 0.1))
-        for i in range(3):
-            p.w_last_edges[i] = float(o["w_last_edges"][i]) if i < len(o["w_last_edges"]) else 1.0
-        p.incl_emerg_traj = 1 if incl_emerg_traj else 0
-        p.filt_window = int(o["filt_window_width"])
-        for i in range(axm.shape[0]):
-            p.axm_v[i] = axm[i, 0]
-            p.axm_a[i] = axm[i, 1]
-        for i in range(axm.shape[0] - 1):   # slopes exactly as np.interp forms them
-            p.axm_s[i] = (axm[i + 1, 1] - axm[i, 1]) / (axm[i + 1, 0] - axm[i, 0])
 
     # -- buffers -----------------------------------------------------------------------------------------------------------
     @staticmethod

@@ -341,6 +341,32 @@ typedef struct LtplVelBatch {
     double* ax;                /* [n_paths][n_points] (last column 0)                                                    */
 } LtplVelBatch;
 
+/* Stand-alone velocity planner on the caller's paths (ltpl_vel_plan_batch): VpForwardBackward.calc_vel_profile and      */
+/* calc_vel_brake_em (VpForwardBackward.py:194-255) for n_paths paths at once, each with its own length and friction.    */
+/* Vehicle parameters from LtplParams: vel_max, gg_scale, ax_max_machines (n_axm, axm_*), drag_coeff, m_veh,            */
+/* dyn_model_exp, and gg_ax / gg_ay when `gg` is NULL.  Arrays are DEVICE pointers; strides are in elements (float64).  */
+/* The struct carries its own size, as LtplSelect does: a binding with another layout is refused at the call.           */
+#define LTPL_VP_PROFILE 0 /* tph.calc_vel_profile(closed=False): friction times gg_scale, v_max, machine limits, v_end   */
+#define LTPL_VP_BRAKE   1 /* tph.calc_vel_profile_brake: raw friction (no gg_scale), no v_end; zeros after standstill  */
+typedef struct LtplVelPlan {
+    int32_t struct_bytes;      /* sizeof(LtplVelPlan) as the caller compiled it; anything else is refused                */
+    int32_t mode;              /* LTPL_VP_PROFILE or LTPL_VP_BRAKE                                                        */
+    int32_t n_paths, n_points; /* row capacity: n_paths > 0 rows of n_points >= 2 points                                 */
+    const int32_t* n_pts;      /* [n_paths] points of each path, 2 <= n <= n_points; NULL: n_points each.  A length out of */
+                               /* that range (it lies on the device, so the call cannot check it) gives a row of NaN in   */
+                               /* vx and ax; the other rows are planned as usual                                         */
+    const double* kappa;       int64_t kappa_s; /* [n_paths][n_points], row stride >= n_points; points >= n are not read */
+    const double* el;          int64_t el_s;    /* [n_paths][n_points - 1 or more], el[i][p] = distance from p to p + 1, */
+                                                /* row stride >= n_points - 1; points >= n - 1 are not read              */
+    const double* gg;          int64_t gg_s;    /* [n_paths][n_points][2] ax_max, ay_max per point, row stride           */
+                                                /* >= 2 n_points; NULL: params.gg_ax / gg_ay everywhere                   */
+    const double* v_start;     /* [n_paths]                                                                              */
+    const double* v_end;       /* [n_paths] (LTPL_VP_PROFILE only; may be NULL for LTPL_VP_BRAKE)                         */
+    double* vx;                /* [n_paths][n_points]                                                                    */
+    double* ax;                /* [n_paths][n_points] (v[p+1]^2 - v[p]^2) / (2 el[p]), 0 at the last point               */
+    int64_t out_s;             /* row stride of vx and ax, >= n_points; both are 0 behind a path's last point            */
+} LtplVelPlan;
+
 /* Scenario inputs that already live on the device (ltpl_stage_inputs_batch): DEVICE pointers and strides, in elements,  */
 /* of the caller's arrays, read through their strides, so column slices and wider rows need no copy.  Scalars have one   */
 /* stride, [B][..] arrays one per dimension.                                                                             */
@@ -431,8 +457,12 @@ int ltpl_set_subbatches(LtplLattice* lat, int n);
 /* stage 0 k_startpos, 1 k_plan, 2 k_path, 3 k_vel, 4 k_export                                                            */
 int ltpl_launch_stage(int stage, const LtplLattice* lat, const LtplParams* prm, const LtplDims* dims,
                       const LtplBuffers* buf, void* stream);
-/* tph.calc_vel_profile(closed=False, loc_gg mode) over dense arrays                                                     */
+/* tph.calc_vel_profile(closed=False, loc_gg mode) over dense arrays with constant friction: ltpl_vel_plan_batch with    */
+/* LTPL_VP_PROFILE, n_pts and gg NULL and every row stride n_points                                                      */
 int ltpl_velprofile_batch(const LtplParams* prm, const LtplVelBatch* vb, void* stream);
+/* the stand-alone velocity planner (LtplVelPlan), in ONE launch on the stream; bad arguments are refused before it,   */
+/* with the field named                                                                                                  */
+int ltpl_vel_plan_batch(const LtplParams* prm, const LtplVelPlan* vp, void* stream);
 /* scenario inputs from device arrays, in ONE launch on the stream (k_stage): writes the input buffers of `buf` (pos,     */
 /* heading, vel, vel_est, n_obj, obj, zone_sel, n_pred, obj_pred; their const marks what the tick kernels do) with the   */
 /* bytes a host copy of the same arrays writes: obj slots k >= k_src and obj_pred behind the given points zero, n_pred   */
