@@ -96,7 +96,8 @@ class PeerGather(object):
 
     Every rank owns one region of a symmetric-memory buffer on ``dst``: [rows_cap][n_export][7] fp32 rows followed by a
     copy of the packed per-path arrays (BatchPlanner.d_meta_raw: traj_len, traj_id, action_id, traj_row, queue_cnt, ...).
-    ``attach`` points the planner's export buffer (LtplBuffers.traj) at the peer region, so the exporting kernels store
+    ``attach`` binds the planner's export rows (LtplBuffers.traj) to the peer region through
+    BatchPlanner.set_export_rows, which every later binding keeps until ``detach``, so the exporting kernels store
     their rows over NVLink while they compute them -- the compact row index comes from the rank-local counter, only
     live rows move.  ``finish`` (on the planner's stream, after the tick) copies the per-path arrays into the region and
     runs the device-side barrier of the symmetric-memory handle; behind it the consumer may read every region."""
@@ -119,21 +120,18 @@ class PeerGather(object):
         self.rows_bytes = rows_bytes
         self.buf = symm_mem.empty(self.world * self.region_bytes, dtype=torch.uint8, device=planner.device)
         self.hdl = symm_mem.rendezvous(self.buf, group if group is not None else dist.group.WORLD)
-        base = int(self.hdl.buffer_ptrs[dst]) + self.rank * self.region_bytes
-        self.peer_rows_ptr = base
-        # tensor view of this rank's meta slot inside the consumer's buffer (peer memory)
+        # tensor views of this rank's rows and meta slot inside the consumer's buffer (peer memory)
+        self.peer_rows = self.hdl.get_buffer(dst, (self.rows_cap * self.row_bytes,), torch.uint8,
+                                             self.rank * self.region_bytes).view(torch.float32) \
+            .view(self.rows_cap, int(d.n_export), 7)
         self.peer_meta = self.hdl.get_buffer(dst, (self.meta_bytes,), torch.uint8,
                                              self.rank * self.region_bytes + rows_bytes)
-        self._saved = None
 
     def attach(self) -> None:
-        self._saved = self.pl.buf.traj
-        self.pl.buf.traj = self.peer_rows_ptr
+        self.pl.set_export_rows(self.peer_rows)
 
     def detach(self) -> None:
-        if self._saved is not None:
-            self.pl.buf.traj = self._saved
-            self._saved = None
+        self.pl.set_export_rows(None)
 
     def finish(self) -> None:
         self.peer_meta.copy_(self.pl.d_meta_raw, non_blocking=True)

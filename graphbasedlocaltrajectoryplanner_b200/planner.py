@@ -191,11 +191,15 @@ DEFAULT_ONLINE = dict(max_heading_offset=0.8, nmbr_export_points=115, v_max_offs
 
 @dataclass
 class TickState:
-    """what a tick changes on the planner's host side besides the pointer fields (buffers), dims and the buffer dicts.
-    A TickGraph keeps a copy of it per captured state and installs that copy after a replay."""
+    """what a tick changes on the planner's host side besides dims and the buffer dicts, with the flags that choose the
+    optional bindings of buffer_sources.  A TickGraph keeps a copy per captured state and installs it after a replay."""
     in_cur: int = 0                  # the device input copy in use (stateful ticks alternate the two)
-    pos_last: torch.Tensor = None    # `pos` of the input copy the last tick used: buffers.pos_last of a stateful tick
+    pos_last: torch.Tensor = None    # `pos` of the input copy the last tick used; set from the first stateful staging on
     gg_planes_used: bool = False     # the last velocity call ran with gg planes (decides the next tick's prev_gg)
+    gg: bool = False                 # this tick's gg planes are bound (set_local_gg_planes; a friction map binds them too)
+    prev_gg: bool = False            # the last stateful staging kept planes as memory: buffers.prev_gg
+    restart: bool = False            # the last stateful staging had a restart mask: buffers.restart
+    export: int = 0                  # the traj_bufs set the tick exports into (plan_stream's set)
     gg_uploaded: bool = False        # the planes set_local_gg_planes bound last came from host arrays
     zone_key_kept: bool = False      # a staging since allocate(): the next stateful tick applies the zone rule
     zone_key_zero: bool = True       # the device zone keys (_zone_key) are all zero
@@ -204,6 +208,34 @@ class TickState:
     ticked: bool = False             # the buffers hold a tick (a velocity call ran since they were allocated)
     emerg: bool = False              # the last velocity call ran with incl_emerg_traj ('emergency' for select)
     selected: bool = False           # select() ran since the last velocity call: sel_action="selected" may be staged
+
+
+SWAPPED = ("path", "node_idx", "nodes", "coeff", "s_vx_ax", "em_vx")            # stateful memory swapped by pointer
+CARRIED = ("action_id", "traj_len", "em_info", "path_len", "n_nodes", "trim")  # stateful memory carried by ONE copy
+_PER_BATCH = tuple(n for n in capi.BUFFER_FIELDS if n not in capi.STATE_FIELDS and n != "traj")
+
+
+def buffer_sources(t: dict, state: dict, traj_bufs: list, tick: TickState, gg_map=None, traj_base=None,
+                   export_rows=None) -> dict:
+    """the tensor behind every field of capi.BUFFER_FIELDS (None: NULL), the one rule for what BatchPlanner passes, from
+    its tables -- ``t`` (the batch's buffers and input copy in use), the memory ``state`` (None without), the export
+    sets, map, id counter and export override when set -- and the flags of ``tick`` that choose optional bindings."""
+    src = dict.fromkeys(capi.BUFFER_FIELDS)
+    src.update((n, t[n]) for n in _PER_BATCH)   # inputs, outputs, scratch; obj_pred and zone_bits may be placeholders
+    src["traj"] = traj_bufs[tick.export] if export_rows is None else export_rows
+    if tick.gg or gg_map is not None:   # the library evaluates a map into this tick's planes
+        src["gg"] = t["gg"]
+    src["gg_map"], src["traj_base"] = gg_map, traj_base
+    if state is not None:
+        src["trim"], src["em_vx"], src["zone_s0"] = t["trim"], t["em_vx"], state["zone_s0"]
+    if state is not None and tick.pos_last is not None:   # from the first stateful staging on
+        src.update(("prev_" + k, state["other"][k]) for k in SWAPPED)
+        src.update(("prev_" + k, state["prev_small"][k]) for k in CARRIED)
+        src.update((k, state[k]) for k in ("st_info", "vel_plan", "course", "obj_dist"))
+        src["sel_action"], src["t_const"], src["pos_last"] = t["sel_action"], t["t_const"], tick.pos_last
+        src["prev_gg"] = state["other"]["gg"] if tick.prev_gg else None
+        src["restart"] = state["restart"] if tick.restart else None
+    return src
 
 
 class BatchPlanner(object):
@@ -250,7 +282,9 @@ class BatchPlanner(object):
         self.lattice_nodes = int(self.header.num_nodes)
         self.dims = None
         self._k_pred_cap = 0
-        self.buf = None
+        self.buf = capi.Buffers()     # the one struct every call passes, for the planner's life (bound by _bind)
+        self._src = None              # the tensors _bind wrote into buf (buffer_sources)
+        self._export_rows = None      # rows that replace the export set (set_export_rows), or None
         self.t = {}
         self.params = capi.Params()
         self._tick_count = 0
@@ -304,8 +338,19 @@ class BatchPlanner(object):
         views = {name: raw[o:o + nb].view(dt).view(shape) for name, (o, nb, shape, dt) in offs.items()}
         return raw, views
 
-    _IN_NAMES = ("pos", "heading", "vel", "vel_est", "n_obj", "obj", "zone_sel", "n_pred", "sel_action", "t_const",
-                 "obj_pred")
+    def _bind(self, *names) -> None:
+        """writes buffer_sources into self.buf in place: every field, or only ``names`` where nothing else changed"""
+        src = buffer_sources(self.t, self._state, self.traj_bufs, self._tick, self._gg_map, self._traj_base,
+                             self._export_rows)
+        for name in names or capi.BUFFER_FIELDS:
+            setattr(self.buf, name, None if src[name] is None else src[name].data_ptr())
+        self._src = src
+
+    def set_export_rows(self, rows=None) -> None:
+        """the compact export rows (buffers.traj) go to ``rows``, a device tensor [(NSLOT + 1) * B][n_export][7] float32
+        that may be peer memory (parallel.PeerGather), instead of the planner's own export sets; None: back to them"""
+        self._export_rows = rows
+        self._bind("traj")
 
     def _alloc_inputs(self, batch: int, k_obj: int, k_pred: int) -> None:
         """The scenario inputs live in ONE packed device buffer (one H2D copy per tick) with N_SETS pinned host staging
@@ -339,11 +384,7 @@ class BatchPlanner(object):
 
     def _use_inputs(self, which: int) -> None:
         self._tick.in_cur = which
-        views = self.d_in[which][1]
-        self.t.update(views)
-        for name in self._IN_NAMES:
-            if name in views and name not in ("sel_action", "t_const"):
-                setattr(self.buf, name, views[name].data_ptr())
+        self.t.update(self.d_in[which][1])
 
     @property
     def _in_cur(self) -> int:
@@ -362,6 +403,7 @@ class BatchPlanner(object):
             # more object slots / prediction points than before: only the input buffers grow (see _alloc_inputs)
             torch.cuda.current_stream(self.device).synchronize()
             self._alloc_inputs(batch, max(k_obj, self.dims.k_obj), max(int(k_pred), self._k_pred_cap))
+            self._bind()
             self._generation += 1
             return
         d = capi.Dims()
@@ -390,17 +432,12 @@ class BatchPlanner(object):
             s_vx_ax=z((3, NSLOT * B, P), f64),
             traj=z(((NSLOT + 1) * B, NE, 7), f32))
         t.update(t_meta)
-        buf = capi.Buffers()
         t["zone_bits"] = torch.zeros((1, 1), dtype=torch.int32, device=dev)   # replaced by _stage_zones()
         d.k_pred = 0
         d.n_zones, d.n_zone_words = 0, (self.lattice_nodes + 31) // 32
-        for name in capi.BUFFER_FIELDS:
-            if name not in capi.STATE_FIELDS and name in t:   # `trim` is a state field: NULL unless the planner is stateful
-                setattr(buf, name, t[name].data_ptr())
-        self.t, self.buf, self.dims = t, buf, d
+        self.t, self.dims = t, d
+        self._export_rows = None   # sized for the old batch
         self._generation += 1
-        if self._traj_base is not None:
-            buf.traj_base = self._traj_base.data_ptr()
         self._tick = TickState()
         # zone keys of the last staged batch, which the next stateful tick compares with (k_stage reads and writes them);
         # one buffer per allocation, so that captured graphs keep its address
@@ -423,7 +460,9 @@ class BatchPlanner(object):
         self._row_bytes = NE * 7 * 4
         if self._stateful:
             self._alloc_state()   # incl. zone_s0, which the FIRST tick has to fill
-        self._bind_gg_map()
+        if self._gg_map is not None:
+            self._gg_planes(t)
+        self._bind()
 
     def set_local_gg_planes(self, ax=None, ay=None) -> None:
         """location dependent friction (calc_vel_profile(local_gg={action: [ndarray(P, 2)]}), OTH:649-666) for the batch:
@@ -435,43 +474,33 @@ class BatchPlanner(object):
         on the device along device_results()["path"]): they are copied into this tick's planes on the current stream,
         without a host synchronisation, and give the bytes of the same values as NumPy arrays.  Such tensors are
         checked (device, dtype, shape) before anything changes; a refusal raises ValueError."""
+        B, P = self.dims.batch, self.dims.p_max
         on_device = isinstance(ax, torch.Tensor) or isinstance(ay, torch.Tensor)
         if on_device:
-            check_gg_planes(ax, ay, self.dims.batch, self.dims.p_max, self.device)
-        if self._gg_map is not None:   # captured graphs evaluate the map: they go stale with it
-            self._generation += 1
-        self._gg_map = None
-        self.buf.gg_map = None
-        if ax is None:
-            self._generation += 1
-            self._plane_bumps += 1
-            self._split_pending = None
-            self.buf.gg = None
-            return
-        B, P = self.dims.batch, self.dims.p_max
-        if not on_device:
+            check_gg_planes(ax, ay, B, P, self.device)
+        elif ax is not None:
             ax = np.asarray(ax, dtype=np.float64)
             ay = np.asarray(ay, dtype=np.float64)
             if ax.shape != ay.shape or ax.ndim != 3 or ax.shape[:2] != (NSLOT, B) or ax.shape[2] > P:
                 raise ValueError("local_gg planes must have the shape [NSLOT][B][P <= p_max]")
-        self._generation += 1
+        self._generation += 1 if self._gg_map is None else 2   # captured graphs evaluate a map: they go stale with it
+        self._gg_map = None
         self._plane_bumps += 1
         self._split_pending = None
-        self._tick.gg_uploaded = not on_device
-        planes = self._gg_planes(self.t)
+        self._tick.gg, self._tick.gg_uploaded = ax is not None, ax is not None and not on_device
         if on_device:   # the given values, then 1.0 behind them: what the host path writes
             n = ax.shape[2]
-            rows = planes.view(2, NSLOT, B, P)
+            rows = self._gg_planes(self.t).view(2, NSLOT, B, P)
             rows[0, :, :, :n].copy_(ax)
             rows[1, :, :, :n].copy_(ay)
             if n < P:
                 rows[:, :, :, n:].fill_(1.0)
-            self.buf.gg = planes.data_ptr()
-            return
-        host = np.ones((2, NSLOT * B, P))
-        host[0, :, :ax.shape[2]] = ax.reshape(NSLOT * B, -1)
-        host[1, :, :ay.shape[2]] = ay.reshape(NSLOT * B, -1)
-        self.buf.gg = planes.copy_(torch.from_numpy(host)).data_ptr()
+        elif ax is not None:
+            host = np.ones((2, NSLOT * B, P))
+            host[0, :, :ax.shape[2]] = ax.reshape(NSLOT * B, -1)
+            host[1, :, :ay.shape[2]] = ay.reshape(NSLOT * B, -1)
+            self._gg_planes(self.t).copy_(torch.from_numpy(host))
+        self._bind("gg", "gg_map")
 
     def set_gg_map(self, ax=None, ay=None, x0: float = 0.0, y0: float = 0.0, cell: float = 1.0) -> None:
         """location dependent friction from a map of the track surface, for the whole batch: ``ax``, ``ay`` [ny][nx] =
@@ -482,36 +511,27 @@ class BatchPlanner(object):
         section 7), as calc_vel_profile(local_gg={action: [map(path[:, 0:2])]}) would take it.  The map is uploaded once
         and stays until it is changed.  None: back to the constant tuple of set_vel_params().  Clears the planes of
         set_local_gg_planes().  Bad input raises ValueError and changes nothing."""
-        if ax is None:
-            self._generation += 1
-            self._gg_map = None
-            if self.buf is not None:
-                self.buf.gg_map = None
-                self.buf.gg = None
-            return
-        for a in (ax, ay):
-            if isinstance(a, torch.Tensor) and a.device != self.device:
-                raise ValueError("gg map: a torch tensor must be on the planner's device %s, got %s" % (self.device,
-                                                                                                     a.device))
-        if not isinstance(ax, torch.Tensor):
-            ax = np.asarray(ax, dtype=np.float64)
-        if not isinstance(ay, torch.Tensor):
-            ay = np.asarray(ay, dtype=np.float64)
-        nx, ny, inv_cell = check_gg_map(ax, ay, x0, y0, cell)
-        dev = lambda a: torch.as_tensor(a, dtype=torch.float64).to(self.device)   # noqa: E731
-        self._gg_map = torch.stack((dev(ax), dev(ay)), dim=-1).contiguous()   # [ny][nx][2]: one 16-byte load per vertex
-        p = self.params
-        p.gg_map_x0, p.gg_map_y0, p.gg_map_inv_cell = float(x0), float(y0), inv_cell
-        p.gg_map_nx, p.gg_map_ny = nx, ny
+        if ax is not None:
+            for a in (ax, ay):
+                if isinstance(a, torch.Tensor) and a.device != self.device:
+                    raise ValueError("gg map: a torch tensor must be on the planner's device %s, got %s"
+                                     % (self.device, a.device))
+            if not isinstance(ax, torch.Tensor):
+                ax = np.asarray(ax, dtype=np.float64)
+            if not isinstance(ay, torch.Tensor):
+                ay = np.asarray(ay, dtype=np.float64)
+            nx, ny, inv_cell = check_gg_map(ax, ay, x0, y0, cell)
+            dev = lambda a: torch.as_tensor(a, dtype=torch.float64).to(self.device)   # noqa: E731
+            ax = torch.stack((dev(ax), dev(ay)), dim=-1).contiguous()   # [ny][nx][2]: one 16-byte load per vertex
+            p = self.params
+            p.gg_map_x0, p.gg_map_y0, p.gg_map_inv_cell = float(x0), float(y0), inv_cell
+            p.gg_map_nx, p.gg_map_ny = nx, ny
+        self._gg_map, self._tick.gg = ax, False
         self._generation += 1
-        self._bind_gg_map()
-
-    def _bind_gg_map(self) -> None:
-        """buffers.gg_map and the gg planes the library fills from it (allocated with the other buffers)"""
-        if self._gg_map is None or self.buf is None:
-            return
-        self.buf.gg = self._gg_planes(self.t).data_ptr()
-        self.buf.gg_map = self._gg_map.data_ptr()
+        if self.dims is not None:   # (allocate binds them otherwise)
+            if ax is not None:   # the planes the library evaluates the map into
+                self._gg_planes(self.t)
+            self._bind("gg", "gg_map")
 
     def _gg_planes(self, planes: dict) -> torch.Tensor:
         """``planes["gg"]``: the gg planes [2][NSLOT * B][p_max] of this batch (this tick's in ``t``, the last tick's in
@@ -632,7 +652,7 @@ class BatchPlanner(object):
         if key != self._tick.zones:
             bits = torch.from_numpy(self._zone_bits(zones)).pin_memory()
             self.t["zone_bits"] = bits.to(self.device, non_blocking=True)
-            self.buf.zone_bits = self.t["zone_bits"].data_ptr()
+            self._bind("zone_bits")
             self._tick.zones = key
         self.dims.n_zones = len(zones)
 
@@ -766,15 +786,11 @@ class BatchPlanner(object):
         stream.synchronize()
         n = int(out["queue_cnt"][2])
         if n:
-            out["traj"][:n].copy_(self._traj_buf()[:n], non_blocking=True)
+            out["traj"][:n].copy_(self._src["traj"][:n], non_blocking=True)
             stream.synchronize()   # the caller reads pinned host memory: the copy has to be complete
         out["n_rows"] = n
         out["incl_emerg_traj"] = bool(self.params.incl_emerg_traj)
         return out
-
-    def _traj_buf(self) -> torch.Tensor:
-        """the compact export buffer of traj_bufs that buffers.traj points at (the one the last tick wrote)"""
-        return next(tb for tb in self.traj_bufs if tb.data_ptr() == self.buf.traj)
 
     def plan_stream(self, batches, vel_est=None, device_hook=None, prefer=None):
         """Pipelined end-to-end planning of a sequence of ScenarioBatch objects (generator of result dicts, in order).
@@ -840,7 +856,8 @@ class BatchPlanner(object):
                 if device_hook is not None and hasattr(device_hook, "before"):
                     device_hook.before(k)   # e.g. wait until a collective that still reads buffer set k has finished
                 self.stage_scenarios(sc, vel_est=vel_est, which=k)
-                self.buf.traj = self.traj_bufs[k].data_ptr()
+                self._tick.export = k
+                self._bind("traj")
                 self.upload(which=k)
                 self.set_startpos()
                 self.tick()
@@ -859,8 +876,9 @@ class BatchPlanner(object):
                 ev_d2h[j].synchronize()
                 yield results[j]
         finally:
-            if self.buf is not None:   # (a refusal may come before the first batch allocated anything)
-                self.buf.traj = self.traj_bufs[0].data_ptr()
+            if self.dims is not None:   # (a refusal may come before the first batch allocated anything)
+                self._tick.export = 0
+                self._bind("traj")
 
     # -- kernels ---------------------------------------------------------------------------------------------------------------
     def _call(self, name):
@@ -890,7 +908,7 @@ class BatchPlanner(object):
         return self._select(self._prefer_tensor(prefer), sel_action, 0)
 
     def _check_select(self, what: str) -> None:
-        if self.buf is None or not self._tick.ticked:
+        if not self._tick.ticked:
             raise ValueError("%s: no velocity call ran on this planner's buffers" % what)
         if all(tb.data_ptr() != self.buf.traj for tb in self.traj_bufs):
             raise ValueError("%s: buffers.traj points at peer memory (a PeerGather is attached)" % what)
@@ -965,7 +983,7 @@ class BatchPlanner(object):
         self._tick_count += 1
         self.params.traj_base_id = 10 * self._tick_count if self._traj_base is None else 0
         self._call(name)
-        self._tick.gg_planes_used = self.buf.gg is not None
+        self._tick.gg_planes_used = self._src["gg"] is not None
         self._tick.ticked = True
         self._tick.emerg, self._tick.selected = bool(self.params.incl_emerg_traj), False
 
@@ -983,26 +1001,20 @@ class BatchPlanner(object):
         self._call_vel("ltpl_tick_batch")
 
     # -- stateful tick (DESIGN.md section 11, csrc/ltpl_state.cuh) ----------------------------------------------
-    _BIG = ("path", "node_idx", "nodes", "coeff", "s_vx_ax", "em_vx")            # swapped by pointer
-    _SMALL = ("action_id", "traj_len", "em_info", "path_len", "n_nodes", "trim")  # carried by ONE device copy
-
     def _alloc_state(self) -> None:
         dev, B = self.device, self.dims.batch
         f64, i32 = torch.float64, torch.int32
         z = lambda shape, dt: torch.zeros(shape, dtype=dt, device=dev)   # noqa: E731
         t = self.t
         t["em_vx"] = z((B, self.dims.n_export), f64)   # f64 velocity of the emergency trajectory (executed 'emergency')
-        self.buf.em_vx = t["em_vx"].data_ptr()
         t["em_info"].fill_(-1)
         prev_raw, prev_small = self._packed(self._carry_spec, lambda n: torch.zeros(n, dtype=torch.uint8, device=dev))
         prev_small["em_info"].fill_(-1)
-        st = dict(other={k: torch.zeros_like(t[k]) for k in self._BIG}, prev_raw=prev_raw, prev_small=prev_small,
+        st = dict(other={k: torch.zeros_like(t[k]) for k in SWAPPED}, prev_raw=prev_raw, prev_small=prev_small,
                   st_info=z((B, 8), i32), vel_plan=z((B,), f64), course=z((B, self.dims.n_export), f64),
                   obj_dist=z((B,), f64))
         st["zone_s0"] = torch.full((B,), -1, dtype=i32, device=dev)
         st["restart"] = z((B,), i32)   # buffers.restart of the ticks with a restart mask
-        self.buf.zone_s0 = st["zone_s0"].data_ptr()
-        self.buf.trim = t["trim"].data_ptr()
         self._state = st
 
     def _restart_mask(self, restart):
@@ -1037,34 +1049,23 @@ class BatchPlanner(object):
             restart = self._restart_mask(restart)
         if self._state is None:
             self._alloc_state()
-        st, t, buf = self._state, self.t, self.buf
+        st, t, ts = self._state, self.t, self._tick
         n_carry = st["prev_raw"].numel()
         st["prev_raw"].copy_(self.d_meta_raw[:n_carry])       # the last tick's small per-path arrays
-        for k in self._BIG:                                   # this tick writes the other set, the last one is memory
+        for k in SWAPPED:                                     # this tick writes the other set, the last one is memory
             t[k], st["other"][k] = st["other"][k], t[k]
-            setattr(buf, k, t[k].data_ptr())
-            setattr(buf, "prev_" + k, st["other"][k].data_ptr())
-        for k in self._SMALL:
-            setattr(buf, "prev_" + k, st["prev_small"][k].data_ptr())
         # location dependent local_gg of the last tick = backup for a brake on the old plan (__backup_path_gg, OTH:970)
-        if self._tick.gg_planes_used:
+        if ts.gg_planes_used:
             t["gg"], st["other"]["gg"] = self._gg_planes(st["other"]), t["gg"]
-            buf.prev_gg = st["other"]["gg"].data_ptr()
-        else:
-            buf.prev_gg = None
-        buf.gg = None            # this tick's local_gg arrives with its calc_vel_profile ...
-        self._bind_gg_map()      # ... or from the friction map, into this tick's planes
+        ts.prev_gg = ts.gg_planes_used
+        ts.gg = False   # this tick's local_gg arrives with its calc_vel_profile, or from the friction map
+        ts.restart = restart is not None
         # pos_est of the previous calc_vel_profile (OTH:537) = `pos` of the input copy the last tick used; this tick
         # stages into the other copy (a batch with more objects than before re-creates only the input buffers)
-        self._tick.pos_last = t["pos"]
+        ts.pos_last = t["pos"]
         self._grow_for(sc)
-        self._use_inputs(1 - self._tick.in_cur)
-        buf.pos_last = self._tick.pos_last.data_ptr()
-        for k in ("st_info", "vel_plan", "course", "obj_dist"):
-            setattr(buf, k, st[k].data_ptr())
-        buf.sel_action = t["sel_action"].data_ptr()
-        buf.t_const = t["t_const"].data_ptr()
-        buf.restart = None if restart is None else st["restart"].data_ptr()
+        self._use_inputs(1 - ts.in_cur)
+        self._bind()
         self._stage(sc, vel_est, 0, (sel_action, t_const, restart))
         self.upload()   # a ScenarioBatch: ONE packed H2D copy (k_stage has written a DeviceScenarioBatch)
         if selected is not None and not isinstance(sc, DeviceScenarioBatch):
@@ -1180,23 +1181,22 @@ class BatchPlanner(object):
         self._stage_zones(sc.zones)
         if self._traj_base is None:   # the ids an all-eager session would give next
             self._traj_base = torch.full((1,), 10 * self._tick_count, dtype=torch.int32, device=self.device)
-        self.buf.traj_base = self._traj_base.data_ptr()
         self.params.traj_base_id = 0
-        buf = capi.Buffers.from_buffer_copy(self.buf)
-        if planes:   # the buffers the velocity half will pass
-            buf.gg = self.t["gg"].data_ptr()
-        capi.check(self.lib, self.lib.ltpl_prepare_batch(self.handle, C.byref(self.params), C.byref(self.dims),
-                                                         C.byref(buf)), "ltpl_prepare_batch")
+        ts = self._tick
+        self._tick = replace(ts, gg=ts.gg or planes)   # bound as the velocity half will bind them
+        self._bind()
+        rc = self.lib.ltpl_prepare_batch(self.handle, C.byref(self.params), C.byref(self.dims), C.byref(self.buf))
+        self._tick = ts
+        self._bind("gg")
+        capi.check(self.lib, rc, "ltpl_prepare_batch")
 
     def _host_state(self) -> dict:
-        """what a tick changes on the host: the pointer fields and dims a call passes, the buffer dicts (by reference)
-        and the TickState record"""
-        return dict(buf=capi.Buffers.from_buffer_copy(self.buf), dims=capi.Dims.from_buffer_copy(self.dims),
-                    t=dict(self.t), other=None if self._state is None else dict(self._state["other"]),
-                    tick=replace(self._tick))
+        """what a tick changes on the host: dims, the buffer dicts (by reference) and the TickState record, from which
+        _bind derives the pointer fields"""
+        return dict(dims=capi.Dims.from_buffer_copy(self.dims), t=dict(self.t),
+                    other=None if self._state is None else dict(self._state["other"]), tick=replace(self._tick))
 
     def _set_host_state(self, hs: dict) -> None:
-        C.memmove(C.addressof(self.buf), C.addressof(hs["buf"]), C.sizeof(capi.Buffers))
         C.memmove(C.addressof(self.dims), C.addressof(hs["dims"]), C.sizeof(capi.Dims))
         self.t.clear()
         self.t.update(hs["t"])
@@ -1204,11 +1204,12 @@ class BatchPlanner(object):
             self._state["other"].clear()
             self._state["other"].update(hs["other"])
         self._tick = replace(hs["tick"])   # a copy: the record in hs serves every replay of its graph
+        self._bind()
 
     def _tick_key(self, stateful: bool) -> tuple:
         """the buffers the next tick would use: the input copy, the ping-pong planes, the gg planes and, for a stateful
         tick, whether the last velocity call ran with planes (it decides the gg swap and prev_gg)"""
-        key = (self._tick.in_cur,) + tuple(self.t[k].data_ptr() if k in self.t else 0 for k in self._BIG + ("gg",))
+        key = (self._tick.in_cur,) + tuple(self.t[k].data_ptr() if k in self.t else 0 for k in SWAPPED + ("gg",))
         return key + (self._tick.gg_planes_used,) if stateful else key
 
     def launch_count(self) -> int:
@@ -1229,7 +1230,7 @@ class BatchPlanner(object):
         evaluates them for set_local_gg_planes.  A stateful tick swaps this plane by pointer, so the view belongs to
         the tick that produced it; take device_results() anew after every calc_paths."""
         out = {n: self.t[n] for n in self.DEVICE_RESULTS}
-        out["traj"] = self._traj_buf()
+        out["traj"] = self._src["traj"]
         out["path"] = self.t["path"]
         return out
 

@@ -241,7 +241,7 @@ def _tick_inputs(pl, what: str, stateful: bool, sc, vel_est, sel_action, t_const
     name: the graph stages the planner's selection buffer)"""
     if not isinstance(sc, DeviceScenarioBatch):
         raise ValueError("%s: needs a DeviceScenarioBatch (a host ScenarioBatch is copied on the host every tick)" % what)
-    if pl._gg_map is None and pl.buf is not None and pl.buf.gg is not None and pl._tick.gg_uploaded:
+    if pl._gg_map is None and pl._tick.gg and pl._tick.gg_uploaded:
         raise ValueError("%s: uploaded local_gg planes (set_local_gg_planes) are per-tick host data; a friction map "
                          "(set_gg_map) is evaluated inside the tick" % what)
     if stateful:
