@@ -111,6 +111,21 @@ class VelPlan(C.Structure):
         self.struct_bytes = C.sizeof(VelPlan)
 
 
+class VelFollow(C.Structure):
+    """LtplVelFollow; it carries its size (struct_bytes), which ltpl_vel_follow_batch checks at every call"""
+    _fields_ = [("struct_bytes", C.c_int32), ("n_paths", C.c_int32), ("n_points", C.c_int32), ("n_pts", C.c_void_p),
+                ("kappa", C.c_void_p), ("kappa_s", C.c_int64), ("el", C.c_void_p), ("el_s", C.c_int64),
+                ("gg", C.c_void_p), ("gg_s", C.c_int64), ("v_start", C.c_void_p), ("v_ego", C.c_void_p),
+                ("v_obj", C.c_void_p), ("safety_d", C.c_void_p), ("obj_dist", C.c_void_p), ("obj_pos", C.c_void_p),
+                ("obj_pos_s", C.c_int64), ("glob_rl", C.c_void_p), ("n_glob", C.c_int32), ("veh_length", C.c_double),
+                ("vx", C.c_void_p), ("ax", C.c_void_p), ("out_s", C.c_int64), ("too_close", C.c_void_p),
+                ("vel_bound", C.c_void_p)]
+
+    def __init__(self):
+        super().__init__()
+        self.struct_bytes = C.sizeof(VelFollow)
+
+
 class StageSrc(C.Structure):
     _fields_ = [("pos", C.c_void_p), ("pos_s", C.c_int64 * 2), ("heading", C.c_void_p), ("heading_s", C.c_int64),
                 ("vel", C.c_void_p), ("vel_s", C.c_int64), ("vel_est", C.c_void_p), ("vel_est_s", C.c_int64),
@@ -138,7 +153,8 @@ EXPORTS = ("ltpl_version", "ltpl_last_error", "ltpl_sizeof", "ltpl_max_objects",
            "ltpl_lattice_destroy", "ltpl_set_startpos_batch", "ltpl_calc_paths_batch", "ltpl_calc_vel_profile_batch",
            "ltpl_tick_batch", "ltpl_velprofile_batch", "ltpl_launch_count", "ltpl_launch_stage", "ltpl_next_tick_batch",
            "ltpl_next_calc_paths_batch", "ltpl_next_calc_vel_profile_batch", "ltpl_set_subbatches",
-           "ltpl_stage_inputs_batch", "ltpl_prepare_batch", "ltpl_select_batch", "ltpl_vel_plan_batch")
+           "ltpl_stage_inputs_batch", "ltpl_prepare_batch", "ltpl_select_batch", "ltpl_vel_plan_batch",
+           "ltpl_vel_follow_batch")
 
 
 def build_library(verbose: bool = False) -> str:
@@ -196,6 +212,8 @@ def load_library():
     lib.ltpl_velprofile_batch.restype = C.c_int
     lib.ltpl_vel_plan_batch.argtypes = [C.POINTER(Params), C.POINTER(VelPlan), C.c_void_p]
     lib.ltpl_vel_plan_batch.restype = C.c_int
+    lib.ltpl_vel_follow_batch.argtypes = [C.POINTER(Params), C.POINTER(VelFollow), C.c_void_p]
+    lib.ltpl_vel_follow_batch.restype = C.c_int
     lib.ltpl_stage_inputs_batch.argtypes = [C.POINTER(Dims), C.POINTER(Buffers), C.POINTER(StageSrc), C.c_void_p]
     lib.ltpl_stage_inputs_batch.restype = C.c_int
     lib.ltpl_prepare_batch.argtypes = [C.c_void_p, C.POINTER(Params), C.POINTER(Dims), C.POINTER(Buffers)]

@@ -17,6 +17,7 @@
 #include "ltpl_vel.cuh"
 #include "ltpl_vel_res.cuh"
 #include "ltpl_velprofile.cuh"
+#include "ltpl_velfollow.cuh"
 #include "ltpl_emerg.cuh"
 #include "ltpl_state.cuh"
 #include "ltpl_smooth.cuh"
@@ -715,6 +716,76 @@ int ltpl_vel_plan_batch(const LtplParams* prm, const LtplVelPlan* vp, void* stre
     const int smem = (gg || ragged) ? vd_smem_general(gg) : VD_SMEM_BYTES;
     kFns[kind]<<<grid, 32, smem, st>>>(*prm, vb, a);
     return check_launch("k_velprofile");
+}
+
+static bool misaligned(const void* p, size_t a) { return ((uintptr_t)p) % a != 0; }
+
+int ltpl_vel_follow_batch(const LtplParams* prm, const LtplVelFollow* vf, void* stream) {
+    if (!prm || !vf) return fail("null argument");
+    if (vf->struct_bytes != (int32_t)sizeof(LtplVelFollow))
+        return fail("vel_follow: vf.struct_bytes must be sizeof(LtplVelFollow) (the caller's layout of the struct differs)");
+    if (vf->n_paths <= 0) return fail("vel_follow: vf.n_paths must be > 0");
+    const int n = vf->n_points;
+    if (n < 2) return fail("vel_follow: vf.n_points must be >= 2");
+    if (vf->n_glob < 2) return fail("vel_follow: vf.n_glob must be >= 2");
+    const struct {
+        const void* p;
+        size_t align;
+        const char* msg;
+    } ptrs[] = {
+        {vf->kappa, 8, "vel_follow: vf.kappa must be set and 8-byte aligned"},
+        {vf->el, 8, "vel_follow: vf.el must be set and 8-byte aligned"},
+        {vf->v_start, 8, "vel_follow: vf.v_start must be set and 8-byte aligned"},
+        {vf->v_ego, 8, "vel_follow: vf.v_ego must be set and 8-byte aligned"},
+        {vf->v_obj, 8, "vel_follow: vf.v_obj must be set and 8-byte aligned"},
+        {vf->safety_d, 8, "vel_follow: vf.safety_d must be set and 8-byte aligned"},
+        {vf->obj_dist, 8, "vel_follow: vf.obj_dist must be set and 8-byte aligned"},
+        {vf->obj_pos, 8, "vel_follow: vf.obj_pos must be set and 8-byte aligned"},
+        {vf->glob_rl, 8, "vel_follow: vf.glob_rl must be set and 8-byte aligned"},
+        {vf->vx, 8, "vel_follow: vf.vx must be set and 8-byte aligned"},
+        {vf->ax, 8, "vel_follow: vf.ax must be set and 8-byte aligned"},
+        {vf->too_close, 1, "vel_follow: vf.too_close must be set"},
+        {vf->vel_bound, 1, "vel_follow: vf.vel_bound must be set"},
+    };
+    for (const auto& q : ptrs)
+        if (!q.p || misaligned(q.p, q.align)) return fail(q.msg);
+    if (vf->n_pts && misaligned(vf->n_pts, 4)) return fail("vel_follow: vf.n_pts must be 4-byte aligned");
+    if (vf->gg && misaligned(vf->gg, 8)) return fail("vel_follow: vf.gg must be 8-byte aligned");
+    if (vf->kappa_s < n) return fail("vel_follow: vf.kappa_s must be >= n_points");
+    if (vf->el_s < n) return fail("vel_follow: vf.el_s must be >= n_points (el has the path's n_points entries)");
+    if (vf->gg && vf->gg_s < 2 * (int64_t)n) return fail("vel_follow: vf.gg_s must be >= 2 n_points");
+    if (vf->obj_pos_s < 2) return fail("vel_follow: vf.obj_pos_s must be >= 2");
+    if (vf->out_s < n) return fail("vel_follow: vf.out_s must be >= n_points");
+    if (prm->n_axm < 1 || prm->n_axm > LTPL_MAX_AXM) return fail("params.n_axm out of range");
+    if (prm->axm_v[prm->n_axm - 1] < prm->vel_max)
+        return fail("ax_max_machines has to cover the entire velocity range of the car (i.e. >= v_max)!");
+    if (prm->follow_control_type != 0 && prm->follow_control_type != 1)
+        return fail("params.follow_control_type must be 0 (PD) or 1 (PDtan)");
+    const bool gg = vf->gg != nullptr;
+    const int kind = (prm->dyn_model_exp == 1.0 ? 1 : 0) + (gg ? 2 : 0);
+    static void (*const kFns[4])(LtplParams, LtplVelFollow) = {k_velfollow<false, false>, k_velfollow<true, false>,
+                                                               k_velfollow<false, true>, k_velfollow<true, true>};
+    const int smem = vf_smem(gg);
+    if (smem > 48 * 1024) {   // the attribute belongs to the kernel on the current device: raised once per device
+        static std::atomic<unsigned long long> s_done{0};
+        int dev = 0;
+        if (cudaGetDevice(&dev) != cudaSuccess || dev >= 64) {
+            (void)cudaGetLastError();
+            return fail("vel_follow: no current CUDA device");
+        }
+        if (!(s_done.load() & (1ull << dev))) {
+            std::lock_guard<std::mutex> lock(g_smem_lock);
+            for (int k = 2; k < 4; ++k)
+                if (cudaFuncSetAttribute((const void*)kFns[k], cudaFuncAttributeMaxDynamicSharedMemorySize, smem) !=
+                    cudaSuccess) {
+                    (void)cudaGetLastError();
+                    return fail("k_velfollow: dynamic shared-memory attribute");
+                }
+            s_done.fetch_or(1ull << dev);
+        }
+    }
+    kFns[kind]<<<(vf->n_paths + 31) / 32, 32, smem, static_cast<cudaStream_t>(stream)>>>(*prm, *vf);
+    return check_launch("k_velfollow");
 }
 
 int ltpl_stage_inputs_batch(const LtplDims* dm, const LtplBuffers* bf, const LtplStageSrc* src, void* stream) {

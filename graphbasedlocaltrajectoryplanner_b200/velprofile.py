@@ -2,8 +2,9 @@
 Stand-alone batched velocity planner on the caller's paths (``ltpl_vel_plan_batch`` of the C-ABI).
 
 ``VelocityPlanner`` replaces ``VpForwardBackward`` (graph_ltpl/online_graph/src/VpForwardBackward.py)
-without a lattice: ``calc_vel_profile`` -> ``tph.calc_vel_profile(closed=False)`` (VPFB:194-227) and
-``calc_vel_brake_em`` -> ``tph.calc_vel_profile_brake`` (VPFB:229-255), for N paths at once, each with its own length
+without a lattice: ``calc_vel_profile`` -> ``tph.calc_vel_profile(closed=False)`` (VPFB:194-227),
+``calc_vel_brake_em`` -> ``tph.calc_vel_profile_brake`` (VPFB:229-255) and ``calc_vel_profile_follow`` ->
+``calc_vel_profile_follow`` (VPFB:141-192, ``ltpl_vel_follow_batch``), for N paths at once, each with its own length
 and, optionally, its own friction per point.  ``velprofile_batch_device`` / ``calc_vel_profile_batch`` are the dense
 constant-friction form of BASELINE.json config 5, with the vehicle parameters of a BatchPlanner.
 """
@@ -75,8 +76,8 @@ def calc_vel_profile_batch(planner, kappa: np.ndarray, el_lengths: np.ndarray, v
 
 
 class VelocityPlanner(object):
-    """VpForwardBackward's calc_vel_profile and calc_vel_brake_em on the device, for N paths per call, without a
-    lattice.  One parameter set per instance, as a VpForwardBackward instance holds it (update_dyn_parameters).
+    """VpForwardBackward's calc_vel_profile, calc_vel_brake_em and calc_vel_profile_follow on the device, for N paths
+    per call, without a lattice.  One parameter set per instance, as a VpForwardBackward instance holds it (update_dyn_parameters).
 
     Arrays: ``kappa`` [N][P]; ``el_lengths`` [N][P - 1] (tph's shape) or [N][P]; ``loc_gg`` a tuple (ax_max, ay_max)
     for every point or an array [N][P][2]; ``v_start`` / ``v_end`` [N]; ``n_pts`` [N] points per path (2 <= n <= P,
@@ -91,18 +92,31 @@ class VelocityPlanner(object):
     ValueError before anything is launched."""
 
     def __init__(self, veh_param_dyn_model_exp: float = 1.0, veh_param_dragcoeff: float = 0.85,
-                 veh_param_mass: float = 1000.0, device=None):
+                 veh_param_mass: float = 1000.0, device=None, len_veh=None, follow_control_type=None,
+                 follow_control_params=None, glob_rl=None):
+        """len_veh, follow_control_type ('PD' or 'PDtan'), follow_control_params (k_p, k_d, c_p and, for PDtan, tan_w:
+        the online ini's [FOLLOW] form) and glob_rl (the closed race line [M + 1][5] s, x, y, kappa, vx with its first
+        point repeated at the end, as Lattice.glob_rl stores it) enable calc_vel_profile_follow (VPFB:22-60); all four
+        or none.  The race line is checked and uploaded here, once."""
         self.lib = capi.load_library()
         self.device = torch.device(device if device is not None else "cuda:0")
         self.veh = dict(dyn_model_exp=float(veh_param_dyn_model_exp), drag_coeff=float(veh_param_dragcoeff),
                         m_veh=float(veh_param_mass))
+        self.follow = check_follow_args(len_veh, follow_control_type, follow_control_params, glob_rl)
+        self.glob_rl = None      # device [M][6] s, x, y, kappa, vx, el (CVPF:166)
+        if self.follow is not None:
+            self.glob_rl = torch.from_numpy(self.follow.pop("glob_rl")).to(self.device)
         self.params = None       # set by update_dyn_parameters
         self._brake_params = self._fill(0.0, 1.0, [[0.0, 0.0]])   # the brake mode reads the vehicle parameters only
 
     def _fill(self, vel_max, gg_scale, ax_max_machines):
         from .planner import DEFAULT_ONLINE, fill_vel_params
         params = capi.Params()
-        fill_vel_params(params, DEFAULT_ONLINE, self.veh, vel_max=float(vel_max), gg_scale=float(gg_scale),
+        online = DEFAULT_ONLINE
+        if self.follow is not None:
+            online = dict(DEFAULT_ONLINE, controller_type=self.follow["control_type"],
+                          control_params=self.follow["control_params"])
+        fill_vel_params(params, online, self.veh, vel_max=float(vel_max), gg_scale=float(gg_scale),
                         local_gg=(1.0, 1.0), ax_max_machines=ax_max_machines, safety_d=0.0, incl_emerg_traj=False)
         return params
 
@@ -120,6 +134,104 @@ class VelocityPlanner(object):
     def calc_vel_brake_em(self, kappa, el_lengths, loc_gg, v_start, n_pts=None, out=None):
         """tph.calc_vel_profile_brake with the raw loc_gg, no gg_scale (VPFB:229-255): zeros after standstill"""
         return self._plan(capi.VP_BRAKE, self._brake_params, kappa, el_lengths, loc_gg, v_start, None, n_pts, out)
+
+    def calc_vel_profile_follow(self, kappa, el_lengths, loc_gg, v_start, v_ego, v_obj, safety_d, obj_dist, obj_pos,
+                                n_pts=None, out=None):
+        """calc_vel_profile_follow (VPFB:141-192, CVPF:78-313) with loc_gg * gg_scale, vel_max and ax_max_machines of
+        update_dyn_parameters.  kappa [N][P]; el_lengths [N][P], the path's whole el column as the reference passes it
+        (its last element enters the ego stop distance); loc_gg a tuple or [N][P][2]; v_start, v_ego, v_obj, safety_d,
+        obj_dist [N]; obj_pos [N][2].  Returns (vx, ax, too_close, vel_bound): vx, ax [N][P] as in calc_vel_profile,
+        too_close and vel_bound (vel_bound_fulfilled) bool [N].  out=(vx, ax, too_close, vel_bound) allocates nothing.
+        A path whose device length is out of range gets a row of NaN and both flags False."""
+        if self.follow is None:
+            raise RuntimeError("calc_vel_profile_follow: construct the VelocityPlanner with len_veh, follow_control_type, "
+                               "follow_control_params and glob_rl")
+        if self.params is None:
+            raise RuntimeError("calc_vel_profile_follow: call update_dyn_parameters first")
+        scal = dict(v_start=v_start, v_ego=v_ego, v_obj=v_obj, safety_d=safety_d, obj_dist=obj_dist)
+        on_device = isinstance(kappa, torch.Tensor)
+        if not on_device:
+            kappa, el_lengths, loc_gg, scal, obj_pos, n_pts = self._upload_follow(kappa, el_lengths, loc_gg, scal,
+                                                                                  obj_pos, n_pts)
+        dev = kappa.device
+        if dev.type != "cuda":
+            raise ValueError("kappa: a CUDA tensor or a NumPy array, got a tensor on %s" % dev)
+        if kappa.dim() != 2 or kappa.shape[0] < 1 or kappa.shape[1] < 2:
+            raise ValueError("kappa must be [N >= 1][P >= 2], got %s" % (tuple(kappa.shape),))
+        n, p = kappa.shape
+        gg = None if isinstance(loc_gg, tuple) else loc_gg
+        if gg is None and (len(loc_gg) != 2 or not all(np.isscalar(g) for g in loc_gg)):
+            raise ValueError("loc_gg: a tuple (ax_max, ay_max) or an array [N][P][2]")
+        if isinstance(el_lengths, torch.Tensor) and el_lengths.dim() == 2 and tuple(el_lengths.shape) == (n, p - 1):
+            raise ValueError("el_lengths: calc_vel_profile_follow takes the path's whole el column [N][P] = [%d][%d] "
+                             "(the last element enters the ego stop distance), got [N][P - 1]" % (n, p))
+        arrays = dict(kappa=(kappa, (n, p)), el_lengths=(el_lengths, (n, p)), obj_pos=(obj_pos, (n, 2)))
+        arrays.update({k: (v, (n,)) for k, v in scal.items()})
+        if gg is not None:
+            arrays["loc_gg"] = (gg, (n, p, 2))
+        for name, (t, shape) in arrays.items():
+            if not isinstance(t, torch.Tensor) or t.device != dev or t.dtype != torch.float64 or tuple(t.shape) != shape:
+                raise ValueError("%s: a float64 tensor %s on %s, got %s" % (name, list(shape), dev, _describe(t)))
+        if dev != self.glob_rl.device:
+            raise ValueError("kappa: tensors on %s, the planner's race line is on %s" % (dev, self.glob_rl.device))
+        if n_pts is not None:
+            if not isinstance(n_pts, torch.Tensor) or n_pts.device != dev or n_pts.dtype != torch.int32 \
+                    or tuple(n_pts.shape) != (n,):
+                raise ValueError("n_pts: an int32 tensor [%d] on %s, got %s" % (n, dev, _describe(n_pts)))
+            n_pts = n_pts.contiguous()
+        if out is None:
+            vx = torch.empty((n, p), dtype=torch.float64, device=dev)
+            ax = torch.empty((n, p), dtype=torch.float64, device=dev)
+            too_close = torch.empty(n, dtype=torch.bool, device=dev)
+            vel_bound = torch.empty(n, dtype=torch.bool, device=dev)
+        else:
+            if len(out) != 4:
+                raise ValueError("out: (vx, ax, too_close, vel_bound)")
+            vx, ax, too_close, vel_bound = out
+            for name, t in (("vx", vx), ("ax", ax)):
+                if not isinstance(t, torch.Tensor) or t.device != dev or t.dtype != torch.float64 \
+                        or tuple(t.shape) != (n, p) or t.stride(1) != 1 or t.stride(0) < p:
+                    raise ValueError("out %s: a float64 tensor [%d][%d] on %s with contiguous rows, got %s"
+                                     % (name, n, p, dev, _describe(t)))
+            if vx.stride(0) != ax.stride(0):
+                raise ValueError("out: vx and ax must have the same row stride, got %d and %d"
+                                 % (vx.stride(0), ax.stride(0)))
+            for name, t in (("too_close", too_close), ("vel_bound", vel_bound)):
+                if not isinstance(t, torch.Tensor) or t.device != dev or t.dtype != torch.bool \
+                        or tuple(t.shape) != (n,) or not t.is_contiguous():
+                    raise ValueError("out %s: a contiguous bool tensor [%d] on %s, got %s" % (name, n, dev, _describe(t)))
+        kappa, _ = _rows(kappa, p)
+        el_lengths, _ = _rows(el_lengths, p)
+        if gg is not None:
+            gg, _ = _rows(gg, 2 * p)
+        if obj_pos.stride(-1) != 1 or obj_pos.stride(0) < 2:
+            obj_pos = obj_pos.contiguous()
+        scal = {k: v.contiguous() for k, v in scal.items()}
+        params = self.params
+        if gg is None:
+            params = capi.Params.from_buffer_copy(params)
+            params.gg_ax, params.gg_ay = float(loc_gg[0]), float(loc_gg[1])
+        vf = capi.VelFollow()
+        vf.n_paths, vf.n_points = n, p
+        vf.n_pts = n_pts.data_ptr() if n_pts is not None else None
+        vf.kappa, vf.kappa_s = kappa.data_ptr(), kappa.stride(0)
+        vf.el, vf.el_s = el_lengths.data_ptr(), el_lengths.stride(0)
+        if gg is not None:
+            vf.gg, vf.gg_s = gg.data_ptr(), gg.stride(0)
+        for k, v in scal.items():
+            setattr(vf, k, v.data_ptr())
+        vf.obj_pos, vf.obj_pos_s = obj_pos.data_ptr(), obj_pos.stride(0)
+        vf.glob_rl, vf.n_glob = self.glob_rl.data_ptr(), self.glob_rl.shape[0]
+        vf.veh_length = self.follow["len_veh"]
+        vf.vx, vf.ax, vf.out_s = vx.data_ptr(), ax.data_ptr(), vx.stride(0)
+        vf.too_close, vf.vel_bound = too_close.data_ptr(), vel_bound.data_ptr()
+        stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+        capi.check(self.lib, self.lib.ltpl_vel_follow_batch(C.byref(params), C.byref(vf), stream),
+                   "ltpl_vel_follow_batch")
+        if on_device:
+            return vx, ax, too_close, vel_bound
+        torch.cuda.current_stream(dev).synchronize()
+        return vx.cpu().numpy(), ax.cpu().numpy(), too_close.cpu().numpy(), vel_bound.cpu().numpy()
 
     # -- arguments ---------------------------------------------------------------------------------------------------
     def _plan(self, mode, params, kappa, el, loc_gg, v_start, v_end, n_pts, out):
@@ -180,28 +292,80 @@ class VelocityPlanner(object):
 
     def _upload(self, kappa, el, loc_gg, v_start, v_end, n_pts):
         """NumPy arguments to device tensors; host lengths are checked here, before anything is uploaded"""
-        def host(a, name, dtype=np.float64):
-            if isinstance(a, torch.Tensor):
-                raise ValueError("%s: NumPy arrays and tensors cannot be mixed in one call" % name)
-            a = np.asarray(a)
-            if a.dtype.kind not in "iuf":
-                raise ValueError("%s: a numeric array, got %s" % (name, a.dtype))
-            return np.ascontiguousarray(a, dtype=dtype)
+        h = _host_arrays(kappa, n_pts, el_lengths=el, loc_gg=loc_gg, v_start=v_start, v_end=v_end)
+        return [self._to_device(h[k]) for k in ("kappa", "el_lengths", "loc_gg", "v_start", "v_end", "n_pts")]
 
-        kappa = host(kappa, "kappa")
-        if kappa.ndim != 2 or kappa.shape[0] < 1 or kappa.shape[1] < 2:
-            raise ValueError("kappa must be [N >= 1][P >= 2], got %s" % (kappa.shape,))
-        if n_pts is not None:
-            h = np.asarray(n_pts)
-            if h.dtype.kind not in "iu" or h.shape != (kappa.shape[0],):
-                raise ValueError("n_pts: an integer array [%d], got %s" % (kappa.shape[0], _describe(n_pts)))
-            if np.any(h < 2) or np.any(h > kappa.shape[1]):
-                raise ValueError("n_pts: every length must be in [2, %d], got %d .. %d"
-                                 % (kappa.shape[1], h.min(), h.max()))
-            n_pts = host(h, "n_pts", np.int32)
-        arrays = [kappa, host(el, "el_lengths"), loc_gg if isinstance(loc_gg, tuple) else host(loc_gg, "loc_gg"),
-                  host(v_start, "v_start"), host(v_end, "v_end") if v_end is not None else None, n_pts]
-        return [torch.from_numpy(a).to(self.device) if isinstance(a, np.ndarray) else a for a in arrays]
+    def _upload_follow(self, kappa, el, loc_gg, scal, obj_pos, n_pts):
+        """NumPy arguments of calc_vel_profile_follow to device tensors, all checked on the host first"""
+        h = _host_arrays(kappa, n_pts, el_lengths=el, loc_gg=loc_gg, obj_pos=obj_pos, **scal)
+        k = h["kappa"]
+        if h["el_lengths"].shape == (k.shape[0], k.shape[1] - 1):
+            raise ValueError("el_lengths: calc_vel_profile_follow takes the path's whole el column [N][P] = [%d][%d] "
+                             "(the last element enters the ego stop distance), got [N][P - 1]" % k.shape)
+        d = {name: self._to_device(a) for name, a in h.items()}
+        return d["kappa"], d["el_lengths"], d["loc_gg"], {name: d[name] for name in scal}, d["obj_pos"], d["n_pts"]
+
+    def _to_device(self, a):
+        return torch.from_numpy(a).to(self.device) if isinstance(a, np.ndarray) else a
+
+
+def _host_arrays(kappa, n_pts, **arrays) -> dict:
+    """host checks shared by the NumPy paths: kappa [N >= 1][P >= 2], n_pts (integers in [2, P]) and every other array
+    numeric and not a tensor; returns contiguous float64 arrays (n_pts int32; a loc_gg tuple and None pass through)"""
+    def host(a, name, dtype=np.float64):
+        if isinstance(a, torch.Tensor):
+            raise ValueError("%s: NumPy arrays and tensors cannot be mixed in one call" % name)
+        a = np.asarray(a)
+        if a.dtype.kind not in "iuf":
+            raise ValueError("%s: a numeric array, got %s" % (name, a.dtype))
+        return np.ascontiguousarray(a, dtype=dtype)
+
+    kappa = host(kappa, "kappa")
+    if kappa.ndim != 2 or kappa.shape[0] < 1 or kappa.shape[1] < 2:
+        raise ValueError("kappa must be [N >= 1][P >= 2], got %s" % (kappa.shape,))
+    if n_pts is not None:
+        h = np.asarray(n_pts)
+        if h.dtype.kind not in "iu" or h.shape != (kappa.shape[0],):
+            raise ValueError("n_pts: an integer array [%d], got %s" % (kappa.shape[0], _describe(n_pts)))
+        if np.any(h < 2) or np.any(h > kappa.shape[1]):
+            raise ValueError("n_pts: every length must be in [2, %d], got %d .. %d"
+                             % (kappa.shape[1], h.min(), h.max()))
+        n_pts = host(h, "n_pts", np.int32)
+    out = dict(kappa=kappa, n_pts=n_pts)
+    for name, a in arrays.items():
+        out[name] = a if a is None or (name == "loc_gg" and isinstance(a, tuple)) else host(a, name)
+    return out
+
+
+def check_follow_args(len_veh, control_type, control_params, glob_rl):
+    """the follow arguments of VelocityPlanner: None when none is given, else a dict with the race line in CVPF:166's
+    form [M][6] (s, x, y, kappa, vx, el) as float64 NumPy; ValueError for anything incomplete or malformed"""
+    given = dict(len_veh=len_veh, follow_control_type=control_type, follow_control_params=control_params,
+                 glob_rl=glob_rl)
+    if all(v is None for v in given.values()):
+        return None
+    missing = [k for k, v in given.items() if v is None]
+    if missing:
+        raise ValueError("follow mode needs len_veh, follow_control_type, follow_control_params and glob_rl; missing %s"
+                         % ", ".join(missing))
+    if control_type not in ("PD", "PDtan"):
+        raise ValueError('follow_control_type: "PD" or "PDtan", got %r' % (control_type,))
+    keys = ("k_p", "k_d", "c_p") + (("tan_w",) if control_type == "PDtan" else ())
+    if not isinstance(control_params, dict) or any(k not in control_params for k in keys):
+        raise ValueError("follow_control_params: a dict with %s for %s, got %r" % (", ".join(keys), control_type,
+                                                                                 control_params))
+    cp = {k: float(control_params[k]) for k in keys}
+    g = np.asarray(glob_rl, dtype=np.float64) if not isinstance(glob_rl, torch.Tensor) else None
+    if g is None or g.ndim != 2 or g.shape[0] < 3 or g.shape[1] != 5:
+        raise ValueError("glob_rl: the closed race line [M + 1 >= 3][5] (s, x, y, kappa, vx), got %s"
+                         % _describe(glob_rl))
+    if not np.all(np.isfinite(g)):
+        raise ValueError("glob_rl: every value must be finite")
+    if not np.array_equal(g[-1, 1:3], g[0, 1:3]):
+        raise ValueError("glob_rl: the first point must be repeated at the end (a closed race line, as "
+                         "Lattice.glob_rl stores it)")
+    g6 = np.ascontiguousarray(np.column_stack((g[:-1], np.diff(g[:, 0]))))   # CVPF:166
+    return dict(len_veh=float(len_veh), control_type=control_type, control_params=cp, glob_rl=g6)
 
 
 def _describe(t) -> str:

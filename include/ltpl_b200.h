@@ -367,6 +367,39 @@ typedef struct LtplVelPlan {
     int64_t out_s;             /* row stride of vx and ax, >= n_points; both are 0 behind a path's last point            */
 } LtplVelPlan;
 
+/* Follow-mode velocity profiles on the caller's paths (ltpl_vel_follow_batch): VpForwardBackward.calc_vel_profile_follow */
+/* (VpForwardBackward.py:141-192 -> calc_vel_profile_follow.py:78-313) for n_paths paths at once.  Vehicle parameters    */
+/* from LtplParams: vel_max, gg_scale (on every ego profile, not on the opponent's), ax_max_machines, drag_coeff, m_veh,   */
+/* dyn_model_exp, gg_ax / gg_ay when `gg` is NULL, and the controller follow_control_type, follow_k_p, follow_k_d,        */
+/* follow_c_p, follow_tan_w.  Arrays are DEVICE pointers; strides are in elements.  The struct carries its own size, as   */
+/* LtplVelPlan does.  The library allocates nothing: the caller's vx / ax rows hold the intermediate profiles.           */
+typedef struct LtplVelFollow {
+    int32_t struct_bytes;      /* sizeof(LtplVelFollow) as the caller compiled it; anything else is refused              */
+    int32_t n_paths, n_points; /* row capacity: n_paths > 0 rows of n_points >= 2 points                                 */
+    const int32_t* n_pts;      /* [n_paths] points of each path, 2 <= n <= n_points; NULL: n_points each.  A length out of */
+                               /* range gives a row of NaN in vx and ax and both flags 0                                  */
+    const double* kappa;       int64_t kappa_s; /* [n_paths][n_points], row stride >= n_points                           */
+    const double* el;          int64_t el_s;    /* [n_paths][n_points], row stride >= n_points: el[p] = distance from p  */
+                                                /* to p + 1, and el[n - 1] (the reference's el column) enters the ego    */
+                                                /* stop distance when the brake profile never reaches 0.1 m/s            */
+    const double* gg;          int64_t gg_s;    /* [n_paths][n_points][2] ax_max, ay_max per point, row stride           */
+                                                /* >= 2 n_points; NULL: params.gg_ax / gg_ay everywhere                   */
+    const double* v_start;     /* [n_paths] planned velocity at the path's start                                          */
+    const double* v_ego;       /* [n_paths] estimated ego velocity                                                        */
+    const double* v_obj;       /* [n_paths] velocity of the object followed                                               */
+    const double* safety_d;    /* [n_paths] safety distance                                                               */
+    const double* obj_dist;    /* [n_paths] distance to the object along the path                                         */
+    const double* obj_pos;     int64_t obj_pos_s; /* [n_paths][2] x, y of the object, row stride >= 2                    */
+    const double* glob_rl;     /* [n_glob][6] s, x, y, kappa, vx, el of the closed race line (no repeated point)          */
+    int32_t n_glob;            /* >= 2                                                                                    */
+    double veh_length;         /* vehicle length (both vehicles)                                                          */
+    double* vx;                /* [n_paths][n_points]                                                                    */
+    double* ax;                /* [n_paths][n_points] (v[p+1]^2 - v[p]^2) / (2 el[p]), 0 at the last point               */
+    int64_t out_s;             /* row stride of vx and ax, >= n_points; both are 0 behind a path's last point            */
+    uint8_t* too_close;        /* [n_paths] 1: the object is closer than safety_d + veh_length                           */
+    uint8_t* vel_bound;        /* [n_paths] 1: the profile keeps the velocity bounds (vel_bound_fulfilled)                */
+} LtplVelFollow;
+
 /* Scenario inputs that already live on the device (ltpl_stage_inputs_batch): DEVICE pointers and strides, in elements,  */
 /* of the caller's arrays, read through their strides, so column slices and wider rows need no copy.  Scalars have one   */
 /* stride, [B][..] arrays one per dimension.                                                                             */
@@ -463,6 +496,9 @@ int ltpl_velprofile_batch(const LtplParams* prm, const LtplVelBatch* vb, void* s
 /* the stand-alone velocity planner (LtplVelPlan), in ONE launch on the stream; bad arguments are refused before it,   */
 /* with the field named                                                                                                  */
 int ltpl_vel_plan_batch(const LtplParams* prm, const LtplVelPlan* vp, void* stream);
+/* follow-mode velocity profiles (LtplVelFollow), in ONE launch on the stream; bad arguments are refused before it, with  */
+/* the field named                                                                                                       */
+int ltpl_vel_follow_batch(const LtplParams* prm, const LtplVelFollow* vf, void* stream);
 /* scenario inputs from device arrays, in ONE launch on the stream (k_stage): writes the input buffers of `buf` (pos,     */
 /* heading, vel, vel_est, n_obj, obj, zone_sel, n_pred, obj_pred; their const marks what the tick kernels do) with the   */
 /* bytes a host copy of the same arrays writes: obj slots k >= k_src and obj_pred behind the given points zero, n_pred   */

@@ -95,3 +95,22 @@ print("replayed stateful tick, trajectories:", sum(len(x.get("traj", {})) for x 
 mb = make_velocity_microbench(200, 150, seed=3)
 vx, ax = calc_vel_profile_batch(pl, mb["kappa"], mb["el"], mb["v_start"], mb["v_end"])
 print("dense vx mean", float(np.mean(vx)))
+# follow-mode profiles (k_velfollow): ragged lengths with per-point friction and the race line in shared memory, then
+# constant friction with the race line read through L2 (resampled to 4 x its points, above the shared-memory capacity)
+from tests import vel_follow_ref as R
+from graphbasedlocaltrajectoryplanner_b200.velprofile import VelocityPlanner
+rl = R.race_line()
+fi = R.random_inputs(70, 90, 5, rl)
+fs = np.cumsum(fi["el"], axis=1) - fi["el"]
+fgg = np.stack((4.5 + 0.5 * np.sin(fs / 50.0), 5.0 + 0.5 * np.cos(fs / 70.0)), axis=-1)
+t4 = np.arange(4 * (rl.shape[0] - 1)) / 4.0
+rl4 = np.column_stack([np.interp(t4, np.arange(rl.shape[0]), rl[:, c]) for c in range(5)])
+rl4 = np.vstack((rl4, rl4[:1]))
+rl4[-1, 0] = rl[-1, 0]
+for glob, gg, n_pts in ((rl, fgg, np.random.default_rng(6).integers(2, 91, size=70)), (rl4, (5.0, 5.0), None)):
+    fv = VelocityPlanner(device="cuda:0", veh_param_dyn_model_exp=1.5, len_veh=4.7, follow_control_type="PD",
+                         follow_control_params={"c_p": 1.25, "k_d": 0.025, "k_p": 0.2}, glob_rl=glob)
+    fv.update_dyn_parameters(vel_max=60.0, gg_scale=0.9, ax_max_machines=g["ax_max_machines"])
+    fx, _, ftc, fvb = fv.calc_vel_profile_follow(fi["kappa"], fi["el"], gg, fi["v_start"], fi["v_ego"], fi["v_obj"],
+                                                 fi["safety_d"], fi["obj_dist"], fi["obj_pos"], n_pts=n_pts)
+    print("follow vx mean", float(np.mean(fx)), "too close", int(ftc.sum()), "vel bound", int(fvb.sum()))
