@@ -126,6 +126,20 @@ class VelFollow(C.Structure):
         self.struct_bytes = C.sizeof(VelFollow)
 
 
+class BrakePrefix(C.Structure):
+    """LtplBrakePrefix; it carries its size (struct_bytes), which ltpl_brake_prefix_batch checks at every call"""
+    _fields_ = [("struct_bytes", C.c_int32), ("n_paths", C.c_int32), ("n_points", C.c_int32), ("n_pts", C.c_void_p),
+                ("kappa", C.c_void_p), ("kappa_s", C.c_int64), ("el", C.c_void_p), ("el_s", C.c_int64),
+                ("gg", C.c_void_p), ("gg_s", C.c_int64), ("vel_plan", C.c_void_p), ("vel_course", C.c_void_p),
+                ("vel_course_s", C.c_int64), ("n_course_cap", C.c_int32), ("n_course", C.c_void_p),
+                ("old_gg_scale", C.c_void_p), ("vx_prefix", C.c_void_p), ("vx_prefix_s", C.c_int64),
+                ("n_prefix", C.c_void_p), ("pref_idx", C.c_void_p), ("vel_start", C.c_void_p)]
+
+    def __init__(self):
+        super().__init__()
+        self.struct_bytes = C.sizeof(BrakePrefix)
+
+
 class StageSrc(C.Structure):
     _fields_ = [("pos", C.c_void_p), ("pos_s", C.c_int64 * 2), ("heading", C.c_void_p), ("heading_s", C.c_int64),
                 ("vel", C.c_void_p), ("vel_s", C.c_int64), ("vel_est", C.c_void_p), ("vel_est_s", C.c_int64),
@@ -154,7 +168,7 @@ EXPORTS = ("ltpl_version", "ltpl_last_error", "ltpl_sizeof", "ltpl_max_objects",
            "ltpl_tick_batch", "ltpl_velprofile_batch", "ltpl_launch_count", "ltpl_launch_stage", "ltpl_next_tick_batch",
            "ltpl_next_calc_paths_batch", "ltpl_next_calc_vel_profile_batch", "ltpl_set_subbatches",
            "ltpl_stage_inputs_batch", "ltpl_prepare_batch", "ltpl_select_batch", "ltpl_vel_plan_batch",
-           "ltpl_vel_follow_batch")
+           "ltpl_vel_follow_batch", "ltpl_brake_prefix_batch")
 
 
 def build_library(verbose: bool = False) -> str:
@@ -214,6 +228,8 @@ def load_library():
     lib.ltpl_vel_plan_batch.restype = C.c_int
     lib.ltpl_vel_follow_batch.argtypes = [C.POINTER(Params), C.POINTER(VelFollow), C.c_void_p]
     lib.ltpl_vel_follow_batch.restype = C.c_int
+    lib.ltpl_brake_prefix_batch.argtypes = [C.POINTER(Params), C.POINTER(BrakePrefix), C.c_void_p]
+    lib.ltpl_brake_prefix_batch.restype = C.c_int
     lib.ltpl_stage_inputs_batch.argtypes = [C.POINTER(Dims), C.POINTER(Buffers), C.POINTER(StageSrc), C.c_void_p]
     lib.ltpl_stage_inputs_batch.restype = C.c_int
     lib.ltpl_prepare_batch.argtypes = [C.c_void_p, C.POINTER(Params), C.POINTER(Dims), C.POINTER(Buffers)]

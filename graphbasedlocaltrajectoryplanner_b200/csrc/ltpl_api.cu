@@ -788,6 +788,51 @@ int ltpl_vel_follow_batch(const LtplParams* prm, const LtplVelFollow* vf, void* 
     return check_launch("k_velfollow");
 }
 
+int ltpl_brake_prefix_batch(const LtplParams* prm, const LtplBrakePrefix* bp, void* stream) {
+    if (!prm || !bp) return fail("null argument");
+    if (bp->struct_bytes != (int32_t)sizeof(LtplBrakePrefix))
+        return fail("brake_prefix: bp.struct_bytes must be sizeof(LtplBrakePrefix) (the caller's layout of the struct "
+                    "differs)");
+    if (bp->n_paths <= 0) return fail("brake_prefix: bp.n_paths must be > 0");
+    const int n = bp->n_points;
+    if (n < 2) return fail("brake_prefix: bp.n_points must be >= 2");
+    if (bp->n_course_cap < 0) return fail("brake_prefix: bp.n_course_cap must be >= 0");
+    const struct {
+        const void* p;
+        size_t align;
+        const char* msg;
+    } ptrs[] = {
+        {bp->kappa, 8, "brake_prefix: bp.kappa must be set and 8-byte aligned"},
+        {bp->el, 8, "brake_prefix: bp.el must be set and 8-byte aligned"},
+        {bp->vel_plan, 8, "brake_prefix: bp.vel_plan must be set and 8-byte aligned"},
+        {bp->old_gg_scale, 8, "brake_prefix: bp.old_gg_scale must be set and 8-byte aligned"},
+        {bp->vx_prefix, 8, "brake_prefix: bp.vx_prefix must be set and 8-byte aligned"},
+        {bp->n_prefix, 4, "brake_prefix: bp.n_prefix must be set and 4-byte aligned"},
+        {bp->pref_idx, 4, "brake_prefix: bp.pref_idx must be set and 4-byte aligned"},
+        {bp->vel_start, 8, "brake_prefix: bp.vel_start must be set and 8-byte aligned"},
+    };
+    for (const auto& q : ptrs)
+        if (!q.p || misaligned(q.p, q.align)) return fail(q.msg);
+    if (bp->n_course_cap > 0 && (!bp->vel_course || misaligned(bp->vel_course, 8)))
+        return fail("brake_prefix: bp.vel_course must be set and 8-byte aligned (n_course_cap > 0)");
+    if (bp->n_pts && misaligned(bp->n_pts, 4)) return fail("brake_prefix: bp.n_pts must be 4-byte aligned");
+    if (bp->n_course && misaligned(bp->n_course, 4)) return fail("brake_prefix: bp.n_course must be 4-byte aligned");
+    if (bp->gg && misaligned(bp->gg, 8)) return fail("brake_prefix: bp.gg must be 8-byte aligned");
+    if (bp->kappa_s < n) return fail("brake_prefix: bp.kappa_s must be >= n_points");
+    if (bp->el_s < n - 1) return fail("brake_prefix: bp.el_s must be >= n_points - 1");
+    if (bp->gg && bp->gg_s < 2 * (int64_t)n) return fail("brake_prefix: bp.gg_s must be >= 2 n_points");
+    if (bp->n_course_cap > 0 && bp->vel_course_s < bp->n_course_cap)
+        return fail("brake_prefix: bp.vel_course_s must be >= n_course_cap");
+    if (bp->vx_prefix_s < (int64_t)bp->n_course_cap + n - 1)
+        return fail("brake_prefix: bp.vx_prefix_s must be >= n_course_cap + n_points - 1");
+    if ((int64_t)bp->n_course_cap + n - 1 > INT32_MAX)
+        return fail("brake_prefix: bp.n_course_cap + n_points - 1 must fit in int32");
+    const bool gg = bp->gg != nullptr;
+    (gg ? k_brakeprefix<true> : k_brakeprefix<false>)<<<(bp->n_paths + 31) / 32, 32, vd_smem_prefix(gg),
+                                                         static_cast<cudaStream_t>(stream)>>>(*prm, *bp);
+    return check_launch("k_brakeprefix");
+}
+
 int ltpl_stage_inputs_batch(const LtplDims* dm, const LtplBuffers* bf, const LtplStageSrc* src, void* stream) {
     if (!dm || !bf || !src) return fail("null argument");
     if (dm->batch <= 0 || dm->k_obj < 1) return fail("dims.batch and dims.k_obj must be > 0");

@@ -2,6 +2,8 @@
 // ltpl_velprofile_batch = BASELINE.json config 5):
 //   k_velprofile  tph.calc_vel_profile(closed=False, loc_gg mode), oracle/tph_port.py:463-538 (VPFB:194-227)
 //   k_velbrake    tph.calc_vel_profile_brake, oracle/tph_port.py:659-732 (VPFB:229-255)
+//   k_brakeprefix VpForwardBackward.check_brake_prefix (VPFB:86-139, ltpl_brake_prefix_batch): k_velbrake's chain with
+//                 the old gg scale per path, cut where the speed reaches vel_max
 //
 // Throughput regime (100 k paths x 500 points): one LANE per path, one warp = 32 paths, the path arrays stream through
 // shared memory in tiles of VD_H points x 32 paths (cp.async, transposing on the fly so that a lane reads its path down a
@@ -367,5 +369,146 @@ k_velbrake(const __grid_constant__ LtplParams prm, const __grid_constant__ LtplV
         vd_store_rows(t_v, vb.vx, va.o_s, s_o, path0, p0, lane);
         vd_store_rows(t_a, vb.ax, va.o_s, s_o, path0, p0, lane);
         __syncwarp();
+    }
+}
+
+// k_brakeprefix: k_velbrake's shared memory (kappa, el reused for the prefix values, GG tiles, s_n, s_o), then s_c[32]
+// (course points of each row: where its brake part starts) and s_w[32] (prefix positions from there to the row's end)
+__host__ __device__ constexpr int vd_smem_prefix(bool gg) { return vd_smem_brake(gg) + 64 * 4; }
+
+// points p < lim[r] of row r at base + rs (path0 + r) + off[r] + p: vd_store_rows with a start offset per row
+__device__ __forceinline__ void bp_store_rows(const double* tile, double* base, int64_t rs, const int* off,
+                                              const int* lim, int path0, int p0, int lane) {
+    const int pt = lane % VD_H, sub = lane / VD_H;
+    const int p = p0 + pt;
+#pragma unroll 4
+    for (int r = sub; r < 32; r += 32 / VD_H) {
+        if (p < lim[r]) base[(size_t)(path0 + r) * rs + off[r] + p] = tile[pt * VD_W + r];
+    }
+}
+
+// VpForwardBackward.check_brake_prefix (VPFB:86-139) with the instance's old_gg_scale per path (LtplBrakePrefix).
+// A lane whose vel_plan exceeds vel_max + 0.1 runs k_velbrake's float64 chain (brake_step, friction times its old scale:
+// gx old and 1 / (gy old), as tph reads loc_gg * old_gg_scale) and stops at its cut: the first point at or below vel_max
+// (np.argmax; none, or point 0: n - 1).  Row layout: vel_course[:c] (first pass, through the kappa tile), the brake
+// points [0, idx) from position c on, zeros up to C + n_points - 1.  Tile loads stop once every lane has cut.
+template <bool GG>
+__global__ void __launch_bounds__(32)
+k_brakeprefix(const __grid_constant__ LtplParams prm, const __grid_constant__ LtplBrakePrefix bp) {
+    extern __shared__ __align__(16) unsigned char vd_smem[];
+    double* t_k = reinterpret_cast<double*>(vd_smem);
+    double* t_e = t_k + VD_TILE;
+    double* t_v = t_e;   // the prefix values replace el in place
+    double* t_c = t_k;   // the course passes through the kappa tile before the brake pass
+    double* t_gx = t_e + VD_TILE;
+    double* t_gy = t_gx + VD_TILE;
+    int* s_n = reinterpret_cast<int*>(GG ? t_gy + VD_TILE : t_gx);
+    int* s_o = s_n + 32;
+    int* s_c = s_o + 32;
+    int* s_w = s_c + 32;
+    const int lane = threadIdx.x;
+    const int path0 = blockIdx.x * 32;
+    const int i = path0 + lane;
+    const bool in = i < bp.n_paths;
+    LtplVelBatch vb = {};
+    vb.n_paths = bp.n_paths;
+    vb.n_points = bp.n_points;
+    VdLayout va = {};
+    va.n_pts = bp.n_pts;
+    bool bad;
+    const int n_i = vd_lengths<true>(vb, va, path0, lane, s_n, s_o, bad);
+    const int C = bp.n_course_cap;
+    const int W = C + bp.n_points - 1;   // prefix positions per row
+    int c_i = in ? C : 0;
+    if (in && bp.n_course) c_i = bp.n_course[i];
+    if (in && (c_i < 0 || c_i > C)) bad = true;
+    if (bad) c_i = 0;
+    s_c[lane] = c_i;
+    s_w[lane] = in ? W - c_i : 0;
+    const double vel_max = prm.vel_max;
+    const double vp = in ? bp.vel_plan[i] : 0.0;
+    const double old = in ? bp.old_gg_scale[i] : 1.0;
+    const bool brake = in && !bad && vp > vel_max + 0.1;
+    __syncwarp();
+
+    // ---- vel_course[:c] ----
+    for (int p0 = 0; p0 < C; p0 += VD_H) {
+        vd_load_rows(t_c, bp.vel_course, bp.vel_course_s, 1, s_c, 0, path0, p0, lane);
+        vd_cp_async_wait_all();
+        __syncwarp();
+        vd_store_rows(t_c, bp.vx_prefix, bp.vx_prefix_s, s_c, path0, p0, lane);
+        __syncwarp();
+    }
+
+    // ---- brake points [0, idx) from position c on, then zeros ----
+    const double dmq = prm.drag_coeff / prm.m_veh;
+    const double ax_c = prm.gg_ax * old, iay_c = 1.0 / (prm.gg_ay * old);
+    const double v0 = fmax(vp, 0.0);
+    double w = v0 * v0;
+    bool stopped = false;
+    bool done = !brake;    // the lane has cut (or does not brake)
+    bool nocut = false;    // point 0 is at or below vel_max: np.argmax gives 0, idx = n - 1
+    int idx = 0;
+    double vs = vp;
+    // the cut can fall on point n_points - 1, one behind the last prefix position when C = 0: the loop walks every point
+    // as well as every position (bp_store_rows stores positions < W only)
+    const int ntile = (max(W, bp.n_points) + VD_H - 1) / VD_H;
+    for (int tl = 0; tl < ntile; ++tl) {
+        const int p0 = tl * VD_H;
+        // the inputs of a tile are read while some lane of the warp still brakes inside it
+        if (!__all_sync(LTPL_FULL, done || p0 >= n_i - 1)) {
+            vd_load_rows(t_k, bp.kappa, bp.kappa_s, 1, s_n, 0, path0, p0, lane);
+            vd_load_rows(t_e, bp.el, bp.el_s, 1, s_n, 1, path0, p0, lane);
+            if constexpr (GG) {
+                vd_load_rows(t_gx, bp.gg, bp.gg_s, 2, s_n, 0, path0, p0, lane);
+                vd_load_rows(t_gy, bp.gg + 1, bp.gg_s, 2, s_n, 0, path0, p0, lane);
+            }
+            vd_cp_async_wait_all();
+        }
+        __syncwarp();
+#pragma unroll 1
+        for (int k = 0; k < VD_H; ++k) {
+            const int p = p0 + k;
+            double v = 0.0;
+            if (!done) {
+                v = (p == 0) ? v0 : sqrt(w);
+                if (v <= vel_max && !nocut) {
+                    if (p == 0)
+                        nocut = true;
+                    else
+                        done = true;
+                }
+                if (p == n_i - 1) done = true;
+                if (done) {   // the cut: vx_decel[idx] starts the next profile and is not part of the prefix
+                    idx = p;
+                    vs = v;
+                    v = 0.0;
+                } else if (!stopped) {
+                    const double kabs = fabs(t_k[k * VD_W + lane]), ds = t_e[k * VD_W + lane];
+                    const double nx = GG ? brake_step(w, kabs, t_gx[k * VD_W + lane] * old,
+                                                      1.0 / (t_gy[k * VD_W + lane] * old), prm.dyn_model_exp, dmq, ds)
+                                         : brake_step(w, kabs, ax_c, iay_c, prm.dyn_model_exp, dmq, ds);
+                    if (nx < 0.0)   // negative radicand: standstill, the rest of the profile stays 0
+                        stopped = true;
+                    w = nx < 0.0 ? 0.0 : nx;
+                }
+            }
+            if (bad) v = CUDART_NAN;
+            t_v[k * VD_W + lane] = v;
+        }
+        __syncwarp();
+        bp_store_rows(t_v, bp.vx_prefix, bp.vx_prefix_s, s_c, s_w, path0, p0, lane);
+        __syncwarp();
+    }
+    if (in) {
+        if (bad) {   // the memory stays
+            bp.n_prefix[i] = bp.pref_idx[i] = -1;
+            bp.vel_start[i] = CUDART_NAN;
+        } else {
+            bp.n_prefix[i] = c_i + idx;
+            bp.pref_idx[i] = idx;
+            bp.vel_start[i] = vs;
+            if (!brake) bp.old_gg_scale[i] = prm.gg_scale;
+        }
     }
 }

@@ -3,10 +3,11 @@ Stand-alone batched velocity planner on the caller's paths (``ltpl_vel_plan_batc
 
 ``VelocityPlanner`` replaces ``VpForwardBackward`` (graph_ltpl/online_graph/src/VpForwardBackward.py)
 without a lattice: ``calc_vel_profile`` -> ``tph.calc_vel_profile(closed=False)`` (VPFB:194-227),
-``calc_vel_brake_em`` -> ``tph.calc_vel_profile_brake`` (VPFB:229-255) and ``calc_vel_profile_follow`` ->
-``calc_vel_profile_follow`` (VPFB:141-192, ``ltpl_vel_follow_batch``), for N paths at once, each with its own length
-and, optionally, its own friction per point.  ``velprofile_batch_device`` / ``calc_vel_profile_batch`` are the dense
-constant-friction form of BASELINE.json config 5, with the vehicle parameters of a BatchPlanner.
+``calc_vel_brake_em`` -> ``tph.calc_vel_profile_brake`` (VPFB:229-255), ``calc_vel_profile_follow`` ->
+``calc_vel_profile_follow`` (VPFB:141-192, ``ltpl_vel_follow_batch``) and ``check_brake_prefix`` (VPFB:86-139,
+``ltpl_brake_prefix_batch``), for N paths at once, each with its own length and, optionally, its own friction per point.
+``velprofile_batch_device`` / ``calc_vel_profile_batch`` are the dense constant-friction form of BASELINE.json config 5,
+with the vehicle parameters of a BatchPlanner.
 """
 
 from __future__ import annotations
@@ -76,8 +77,10 @@ def calc_vel_profile_batch(planner, kappa: np.ndarray, el_lengths: np.ndarray, v
 
 
 class VelocityPlanner(object):
-    """VpForwardBackward's calc_vel_profile, calc_vel_brake_em and calc_vel_profile_follow on the device, for N paths
-    per call, without a lattice.  One parameter set per instance, as a VpForwardBackward instance holds it (update_dyn_parameters).
+    """VpForwardBackward's calc_vel_profile, calc_vel_brake_em, calc_vel_profile_follow and check_brake_prefix on the
+    device, for N paths per call, without a lattice.  One parameter set per instance, as a VpForwardBackward instance
+    holds it (update_dyn_parameters); the instance's old_gg_scale of check_brake_prefix is a per-path array the caller
+    keeps.
 
     Arrays: ``kappa`` [N][P]; ``el_lengths`` [N][P - 1] (tph's shape) or [N][P]; ``loc_gg`` a tuple (ax_max, ay_max)
     for every point or an array [N][P][2]; ``v_start`` / ``v_end`` [N]; ``n_pts`` [N] points per path (2 <= n <= P,
@@ -233,6 +236,115 @@ class VelocityPlanner(object):
         torch.cuda.current_stream(dev).synchronize()
         return vx.cpu().numpy(), ax.cpu().numpy(), too_close.cpu().numpy(), vel_bound.cpu().numpy()
 
+    def check_brake_prefix(self, vel_plan, vel_course, kappa, el_lengths, loc_gg, old_gg_scale, n_course=None,
+                           n_pts=None, out=None):
+        """VPFB.check_brake_prefix (VPFB:86-139) for N paths, the instance's old_gg_scale kept per path in the caller's
+        ``old_gg_scale`` [N] (float64, updated in place).  Create it filled with the gg_scale of the first
+        update_dyn_parameters call, as the reference's instance sets old_gg_scale on its first update_dyn_parameters
+        (VPFB:78-80); then pass the same array to every later call.
+
+        Per path i, c = n_course[i] (None: C each), n = n_pts[i]: when vel_plan[i] > vel_max + 0.1 (float64), the brake
+        profile tph.calc_vel_profile_brake(loc_gg * old_gg_scale[i], v_start=vel_plan[i]) is cut at idx = the first
+        point at or below vel_max (n - 1 when there is none or it is point 0): vx_prefix = vel_course[:c] followed by
+        the profile's points [0, idx), pref_idx = idx, vel_start = the profile at idx, and old_gg_scale[i] stays.
+        Otherwise vx_prefix = vel_course[:c], pref_idx = 0, vel_start = vel_plan[i] and old_gg_scale[i] = gg_scale.
+
+        vel_plan [N]; vel_course [N][C] (C = 0 allowed); kappa [N][P]; el_lengths [N][P - 1] or [N][P]; loc_gg a tuple
+        or [N][P][2] (before the scale).  Returns (vx_prefix, n_prefix, pref_idx, vel_start): vx_prefix float64
+        [N][C + P - 1], 0 behind n_prefix[i] = c + pref_idx[i]; n_prefix, pref_idx int32 [N]; vel_start float64 [N].
+        out=(vx_prefix, n_prefix, pref_idx, vel_start) allocates nothing.  A device length out of range (n_pts outside
+        [2, P], n_course outside [0, C]) gives a row of NaN, n_prefix = pref_idx = -1, vel_start NaN and leaves the
+        path's old_gg_scale as it was."""
+        if self.params is None:
+            raise RuntimeError("check_brake_prefix: call update_dyn_parameters first")
+        on_device = isinstance(kappa, torch.Tensor)
+        host_memory = None
+        if not on_device:
+            host_memory = old_gg_scale
+            vel_plan, vel_course, kappa, el_lengths, loc_gg, old_gg_scale, n_course, n_pts = self._upload_prefix(
+                vel_plan, vel_course, kappa, el_lengths, loc_gg, old_gg_scale, n_course, n_pts)
+        dev = kappa.device
+        if dev.type != "cuda":
+            raise ValueError("kappa: a CUDA tensor or a NumPy array, got a tensor on %s" % dev)
+        if kappa.dim() != 2 or kappa.shape[0] < 1 or kappa.shape[1] < 2:
+            raise ValueError("kappa must be [N >= 1][P >= 2], got %s" % (tuple(kappa.shape),))
+        n, p = kappa.shape
+        gg = None if isinstance(loc_gg, tuple) else loc_gg
+        if gg is None and (len(loc_gg) != 2 or not all(np.isscalar(g) for g in loc_gg)):
+            raise ValueError("loc_gg: a tuple (ax_max, ay_max) or an array [N][P][2]")
+        if not isinstance(vel_course, torch.Tensor) or vel_course.dim() != 2:
+            raise ValueError("vel_course: a float64 tensor [%d][C] on %s, got %s" % (n, dev, _describe(vel_course)))
+        cap = vel_course.shape[1]
+        el_cols = el_lengths.shape[-1] if isinstance(el_lengths, torch.Tensor) and el_lengths.dim() == 2 \
+            and el_lengths.shape[-1] in (p - 1, p) else p
+        arrays = dict(kappa=(kappa, (n, p)), el_lengths=(el_lengths, (n, el_cols)), vel_plan=(vel_plan, (n,)),
+                      vel_course=(vel_course, (n, cap)), old_gg_scale=(old_gg_scale, (n,)))
+        if gg is not None:
+            arrays["loc_gg"] = (gg, (n, p, 2))
+        for name, (t, shape) in arrays.items():
+            if not isinstance(t, torch.Tensor) or t.device != dev or t.dtype != torch.float64 or tuple(t.shape) != shape:
+                raise ValueError("%s: a float64 tensor %s on %s, got %s" % (name, list(shape), dev, _describe(t)))
+        if not old_gg_scale.is_contiguous():
+            raise ValueError("old_gg_scale: updated in place, so it must be contiguous")
+        lengths = dict(n_pts=n_pts, n_course=n_course)
+        for name, t in lengths.items():
+            if t is not None:
+                if not isinstance(t, torch.Tensor) or t.device != dev or t.dtype != torch.int32 or tuple(t.shape) != (n,):
+                    raise ValueError("%s: an int32 tensor [%d] on %s, got %s" % (name, n, dev, _describe(t)))
+                lengths[name] = t.contiguous()
+        width = cap + p - 1
+        if out is None:
+            vx_prefix = torch.empty((n, width), dtype=torch.float64, device=dev)
+            n_prefix = torch.empty(n, dtype=torch.int32, device=dev)
+            pref_idx = torch.empty(n, dtype=torch.int32, device=dev)
+            vel_start = torch.empty(n, dtype=torch.float64, device=dev)
+        else:
+            if len(out) != 4:
+                raise ValueError("out: (vx_prefix, n_prefix, pref_idx, vel_start)")
+            vx_prefix, n_prefix, pref_idx, vel_start = out
+            if not isinstance(vx_prefix, torch.Tensor) or vx_prefix.device != dev or vx_prefix.dtype != torch.float64 \
+                    or tuple(vx_prefix.shape) != (n, width) or vx_prefix.stride(1) != 1 or vx_prefix.stride(0) < width:
+                raise ValueError("out vx_prefix: a float64 tensor [%d][%d] on %s with contiguous rows, got %s"
+                                 % (n, width, dev, _describe(vx_prefix)))
+            for name, t, dt in (("n_prefix", n_prefix, torch.int32), ("pref_idx", pref_idx, torch.int32),
+                                ("vel_start", vel_start, torch.float64)):
+                if not isinstance(t, torch.Tensor) or t.device != dev or t.dtype != dt or tuple(t.shape) != (n,) \
+                        or not t.is_contiguous():
+                    raise ValueError("out %s: a contiguous %s tensor [%d] on %s, got %s" % (name, dt, n, dev, _describe(t)))
+        kappa, _ = _rows(kappa, p)
+        el_lengths, _ = _rows(el_lengths, el_lengths.shape[1])
+        if gg is not None:
+            gg, _ = _rows(gg, 2 * p)
+        vel_plan = vel_plan.contiguous()
+        params = self.params
+        if gg is None:
+            params = capi.Params.from_buffer_copy(params)
+            params.gg_ax, params.gg_ay = float(loc_gg[0]), float(loc_gg[1])
+        bp = capi.BrakePrefix()
+        bp.n_paths, bp.n_points = n, p
+        bp.n_pts = lengths["n_pts"].data_ptr() if lengths["n_pts"] is not None else None
+        bp.kappa, bp.kappa_s = kappa.data_ptr(), kappa.stride(0)
+        bp.el, bp.el_s = el_lengths.data_ptr(), el_lengths.stride(0)
+        if gg is not None:
+            bp.gg, bp.gg_s = gg.data_ptr(), gg.stride(0)
+        bp.vel_plan = vel_plan.data_ptr()
+        if cap > 0:
+            vel_course, _ = _rows(vel_course, cap)
+            bp.vel_course, bp.vel_course_s = vel_course.data_ptr(), vel_course.stride(0)
+        bp.n_course_cap = cap
+        bp.n_course = lengths["n_course"].data_ptr() if lengths["n_course"] is not None else None
+        bp.old_gg_scale = old_gg_scale.data_ptr()
+        bp.vx_prefix, bp.vx_prefix_s = vx_prefix.data_ptr(), vx_prefix.stride(0)
+        bp.n_prefix, bp.pref_idx, bp.vel_start = n_prefix.data_ptr(), pref_idx.data_ptr(), vel_start.data_ptr()
+        stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+        capi.check(self.lib, self.lib.ltpl_brake_prefix_batch(C.byref(params), C.byref(bp), stream),
+                   "ltpl_brake_prefix_batch")
+        if on_device:
+            return vx_prefix, n_prefix, pref_idx, vel_start
+        torch.cuda.current_stream(dev).synchronize()
+        host_memory[...] = old_gg_scale.cpu().numpy()
+        return vx_prefix.cpu().numpy(), n_prefix.cpu().numpy(), pref_idx.cpu().numpy(), vel_start.cpu().numpy()
+
     # -- arguments ---------------------------------------------------------------------------------------------------
     def _plan(self, mode, params, kappa, el, loc_gg, v_start, v_end, n_pts, out):
         on_device = isinstance(kappa, torch.Tensor)
@@ -304,6 +416,29 @@ class VelocityPlanner(object):
                              "(the last element enters the ego stop distance), got [N][P - 1]" % k.shape)
         d = {name: self._to_device(a) for name, a in h.items()}
         return d["kappa"], d["el_lengths"], d["loc_gg"], {name: d[name] for name in scal}, d["obj_pos"], d["n_pts"]
+
+    def _upload_prefix(self, vel_plan, vel_course, kappa, el, loc_gg, old_gg_scale, n_course, n_pts):
+        """NumPy arguments of check_brake_prefix to device tensors, all checked on the host first; old_gg_scale must be
+        a float64 NumPy array [N] (it is written back after the call)"""
+        h = _host_arrays(kappa, n_pts, el_lengths=el, loc_gg=loc_gg, vel_plan=vel_plan, vel_course=vel_course)
+        n = h["kappa"].shape[0]
+        if h["vel_course"].ndim != 2 or h["vel_course"].shape[0] != n:
+            raise ValueError("vel_course: an array [%d][C], got %s" % (n, _describe(h["vel_course"])))
+        if not isinstance(old_gg_scale, np.ndarray) or old_gg_scale.dtype != np.float64 or old_gg_scale.shape != (n,) \
+                or not old_gg_scale.flags.writeable:
+            raise ValueError("old_gg_scale: a writeable float64 NumPy array [%d] (updated in place), got %s"
+                             % (n, _describe(old_gg_scale)))
+        if n_course is not None:
+            cap = h["vel_course"].shape[1]
+            c = np.asarray(n_course)
+            if c.dtype.kind not in "iu" or c.shape != (n,):
+                raise ValueError("n_course: an integer array [%d], got %s" % (n, _describe(n_course)))
+            if np.any(c < 0) or np.any(c > cap):
+                raise ValueError("n_course: every length must be in [0, %d], got %d .. %d" % (cap, c.min(), c.max()))
+            n_course = np.ascontiguousarray(c, dtype=np.int32)
+        d = {name: self._to_device(a) for name, a in h.items()}
+        return (d["vel_plan"], d["vel_course"], d["kappa"], d["el_lengths"], d["loc_gg"],
+                self._to_device(np.ascontiguousarray(old_gg_scale)), self._to_device(n_course), d["n_pts"])
 
     def _to_device(self, a):
         return torch.from_numpy(a).to(self.device) if isinstance(a, np.ndarray) else a

@@ -400,6 +400,40 @@ typedef struct LtplVelFollow {
     uint8_t* vel_bound;        /* [n_paths] 1: the profile keeps the velocity bounds (vel_bound_fulfilled)                */
 } LtplVelFollow;
 
+/* Brake to a lowered vel_max (ltpl_brake_prefix_batch): VpForwardBackward.check_brake_prefix (VpForwardBackward.py:86-139) */
+/* for n_paths paths at once, the instance's old_gg_scale kept per path in a caller-owned array.  Per path i, with       */
+/* c = n_course[i] and n = n_pts[i]: when vel_plan[i] > vel_max + 0.1 (float64), the brake profile of                    */
+/* tph.calc_vel_profile_brake from vel_plan[i] with every friction value times old_gg_scale[i] is cut at                  */
+/* idx = the first point whose velocity is <= vel_max (n - 1 when there is none or it is point 0):                       */
+/* vx_prefix = vel_course[:c] followed by the profile's points [0, idx), pref_idx = idx, vel_start = its point idx, and */
+/* old_gg_scale[i] stays.  Otherwise vx_prefix = vel_course[:c], pref_idx = 0, vel_start = vel_plan[i] and              */
+/* old_gg_scale[i] = gg_scale.  Parameters from LtplParams: vel_max, gg_scale, dyn_model_exp, drag_coeff, m_veh, and     */
+/* gg_ax / gg_ay when `gg` is NULL.  Arrays are DEVICE pointers; strides are in elements.  The struct carries its own    */
+/* size, as LtplVelPlan does.  The library allocates nothing.                                                            */
+typedef struct LtplBrakePrefix {
+    int32_t struct_bytes;      /* sizeof(LtplBrakePrefix) as the caller compiled it; anything else is refused            */
+    int32_t n_paths, n_points; /* row capacity: n_paths > 0 rows of n_points >= 2 points                                 */
+    const int32_t* n_pts;      /* [n_paths] points of each path, 2 <= n <= n_points; NULL: n_points each                  */
+    const double* kappa;       int64_t kappa_s; /* [n_paths][n_points], row stride >= n_points                           */
+    const double* el;          int64_t el_s;    /* [n_paths][n_points - 1 or more], row stride >= n_points - 1           */
+    const double* gg;          int64_t gg_s;    /* [n_paths][n_points][2] ax_max, ay_max per point (before the scale),   */
+                                                /* row stride >= 2 n_points; NULL: params.gg_ax / gg_ay everywhere       */
+    const double* vel_plan;    /* [n_paths] velocity of the last plan at the path's start                                 */
+    const double* vel_course;  int64_t vel_course_s; /* [n_paths][n_course_cap] the kept velocity course of the last      */
+                                                     /* trajectory, row stride >= n_course_cap; may be NULL when the      */
+                                                     /* capacity is 0                                                     */
+    int32_t n_course_cap;      /* C >= 0: course capacity per row                                                        */
+    const int32_t* n_course;   /* [n_paths] course points of each path, 0 <= c <= C; NULL: C each                          */
+    double* old_gg_scale;      /* [n_paths] read and written: the gg scale of the path's last call that needed no brake  */
+    double* vx_prefix;         int64_t vx_prefix_s; /* [n_paths][C + n_points - 1], row stride >= C + n_points - 1;     */
+                                                    /* 0 behind n_prefix[i]                                            */
+    int32_t* n_prefix;         /* [n_paths] c + pref_idx                                                                 */
+    int32_t* pref_idx;         /* [n_paths] brake points in the prefix (0: no brake)                                     */
+    double* vel_start;         /* [n_paths] start velocity of the profile that follows the prefix                       */
+                               /* A device length out of range (n_pts outside [2, n_points] or n_course outside [0, C])  */
+                               /* gives a row of NaN, n_prefix = pref_idx = -1, vel_start NaN and leaves old_gg_scale[i]  */
+} LtplBrakePrefix;
+
 /* Scenario inputs that already live on the device (ltpl_stage_inputs_batch): DEVICE pointers and strides, in elements,  */
 /* of the caller's arrays, read through their strides, so column slices and wider rows need no copy.  Scalars have one   */
 /* stride, [B][..] arrays one per dimension.                                                                             */
@@ -499,6 +533,9 @@ int ltpl_vel_plan_batch(const LtplParams* prm, const LtplVelPlan* vp, void* stre
 /* follow-mode velocity profiles (LtplVelFollow), in ONE launch on the stream; bad arguments are refused before it, with  */
 /* the field named                                                                                                       */
 int ltpl_vel_follow_batch(const LtplParams* prm, const LtplVelFollow* vf, void* stream);
+/* brake prefixes to a lowered vel_max (LtplBrakePrefix), in ONE launch on the stream; bad arguments are refused before  */
+/* it, with the field named                                                                                              */
+int ltpl_brake_prefix_batch(const LtplParams* prm, const LtplBrakePrefix* bp, void* stream);
 /* scenario inputs from device arrays, in ONE launch on the stream (k_stage): writes the input buffers of `buf` (pos,     */
 /* heading, vel, vel_est, n_obj, obj, zone_sel, n_pred, obj_pred; their const marks what the tick kernels do) with the   */
 /* bytes a host copy of the same arrays writes: obj slots k >= k_src and obj_pred behind the given points zero, n_pred   */

@@ -114,3 +114,14 @@ for glob, gg, n_pts in ((rl, fgg, np.random.default_rng(6).integers(2, 91, size=
     fx, _, ftc, fvb = fv.calc_vel_profile_follow(fi["kappa"], fi["el"], gg, fi["v_start"], fi["v_ego"], fi["v_obj"],
                                                  fi["safety_d"], fi["obj_dist"], fi["obj_pos"], n_pts=n_pts)
     print("follow vx mean", float(np.mean(fx)), "too close", int(ftc.sum()), "vel bound", int(fvb.sum()))
+# brake prefixes (k_brakeprefix): ragged paths and courses with per-point friction, then constant friction; about half
+# of the paths brake, the memory differs from gg_scale
+bv = VelocityPlanner(device="cuda:0")
+bv.update_dyn_parameters(vel_max=30.0, gg_scale=0.9, ax_max_machines=g["ax_max_machines"])
+brng = np.random.default_rng(8)
+bplan = np.where(brng.random(70) < 0.5, brng.uniform(31.0, 70.0, size=70), brng.uniform(0.0, 30.0, size=70))
+for gg, n_pts in ((fgg, np.random.default_rng(9).integers(2, 91, size=70)), ((5.0, 5.0), None)):
+    bold = brng.uniform(0.5, 1.0, size=70)
+    bx, bn, bi, bs = bv.check_brake_prefix(bplan, brng.uniform(10.0, 60.0, size=(70, 4)), fi["kappa"], fi["el"], gg,
+                                           bold, n_course=brng.integers(0, 5, size=70), n_pts=n_pts)
+    print("brake prefix mean", float(np.mean(bx)), "braking", int((bi > 0).sum()), "n_prefix", int(bn.sum()))
