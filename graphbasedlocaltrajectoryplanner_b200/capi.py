@@ -140,6 +140,24 @@ class BrakePrefix(C.Structure):
         self.struct_bytes = C.sizeof(BrakePrefix)
 
 
+PC_S_COORD, PC_S_INDEX, PC_CLOSEST, PC_INSIDE_BOUNDS = 0, 1, 2, 3   # LtplPathCoord.mode
+
+
+class PathCoord(C.Structure):
+    """LtplPathCoord; it carries its size (struct_bytes), which ltpl_path_coord_batch checks at every call"""
+    _fields_ = [("struct_bytes", C.c_int32), ("mode", C.c_int32), ("closed", C.c_int32), ("n_queries", C.c_int32),
+                ("m_points", C.c_int32), ("x", C.c_void_p), ("y", C.c_void_p), ("line_s", C.c_int64),
+                ("pt_s", C.c_int64), ("x2", C.c_void_p), ("y2", C.c_void_p), ("line2_s", C.c_int64),
+                ("pt2_s", C.c_int64), ("s_array", C.c_void_p), ("s_array_s", C.c_int64), ("s_array_es", C.c_int64),
+                ("pos", C.c_void_p),
+                ("pos_s", C.c_int64 * 2), ("n_pts", C.c_void_p), ("s", C.c_void_p), ("closest", C.c_void_p),
+                ("idx", C.c_void_p), ("inside", C.c_void_p)]
+
+    def __init__(self):
+        super().__init__()
+        self.struct_bytes = C.sizeof(PathCoord)
+
+
 class StageSrc(C.Structure):
     _fields_ = [("pos", C.c_void_p), ("pos_s", C.c_int64 * 2), ("heading", C.c_void_p), ("heading_s", C.c_int64),
                 ("vel", C.c_void_p), ("vel_s", C.c_int64), ("vel_est", C.c_void_p), ("vel_est_s", C.c_int64),
@@ -168,7 +186,7 @@ EXPORTS = ("ltpl_version", "ltpl_last_error", "ltpl_sizeof", "ltpl_max_objects",
            "ltpl_tick_batch", "ltpl_velprofile_batch", "ltpl_launch_count", "ltpl_launch_stage", "ltpl_next_tick_batch",
            "ltpl_next_calc_paths_batch", "ltpl_next_calc_vel_profile_batch", "ltpl_set_subbatches",
            "ltpl_stage_inputs_batch", "ltpl_prepare_batch", "ltpl_select_batch", "ltpl_vel_plan_batch",
-           "ltpl_vel_follow_batch", "ltpl_brake_prefix_batch")
+           "ltpl_vel_follow_batch", "ltpl_brake_prefix_batch", "ltpl_path_coord_batch")
 
 
 def build_library(verbose: bool = False) -> str:
@@ -230,6 +248,8 @@ def load_library():
     lib.ltpl_vel_follow_batch.restype = C.c_int
     lib.ltpl_brake_prefix_batch.argtypes = [C.POINTER(Params), C.POINTER(BrakePrefix), C.c_void_p]
     lib.ltpl_brake_prefix_batch.restype = C.c_int
+    lib.ltpl_path_coord_batch.argtypes = [C.POINTER(PathCoord), C.c_void_p]
+    lib.ltpl_path_coord_batch.restype = C.c_int
     lib.ltpl_stage_inputs_batch.argtypes = [C.POINTER(Dims), C.POINTER(Buffers), C.POINTER(StageSrc), C.c_void_p]
     lib.ltpl_stage_inputs_batch.restype = C.c_int
     lib.ltpl_prepare_batch.argtypes = [C.c_void_p, C.POINTER(Params), C.POINTER(Dims), C.POINTER(Buffers)]

@@ -25,6 +25,7 @@
 #include "ltpl_stage.cuh"
 #include "ltpl_traj_base.cuh"
 #include "ltpl_select.cuh"
+#include "ltpl_pathcoord.cuh"
 
 // the memory records are the int32 arrays BatchPlanner allocates: st_info [B][8], trim [NSLOT*B][4]
 static_assert(sizeof(LtplStateInfo) == 8 * sizeof(int32_t) && alignof(LtplStateInfo) == alignof(int32_t), "st_info row");
@@ -831,6 +832,60 @@ int ltpl_brake_prefix_batch(const LtplParams* prm, const LtplBrakePrefix* bp, vo
     (gg ? k_brakeprefix<true> : k_brakeprefix<false>)<<<(bp->n_paths + 31) / 32, 32, vd_smem_prefix(gg),
                                                          static_cast<cudaStream_t>(stream)>>>(*prm, *bp);
     return check_launch("k_brakeprefix");
+}
+
+int ltpl_path_coord_batch(const LtplPathCoord* pc, void* stream) {
+    if (!pc) return fail("null argument");
+    if (pc->struct_bytes != (int32_t)sizeof(LtplPathCoord))
+        return fail("path_coord: pc.struct_bytes must be sizeof(LtplPathCoord) (the caller's layout of the struct "
+                    "differs)");
+    const int mode = pc->mode;
+    if (mode < LTPL_PC_S_COORD || mode > LTPL_PC_INSIDE_BOUNDS)
+        return fail("path_coord: pc.mode must be LTPL_PC_S_COORD, LTPL_PC_S_INDEX, LTPL_PC_CLOSEST or "
+                    "LTPL_PC_INSIDE_BOUNDS");
+    if (pc->n_queries < 0) return fail("path_coord: pc.n_queries must be >= 0");
+    const int64_t m = pc->m_points;
+    if (m < 2) return fail("path_coord: pc.m_points must be >= 2");
+    if (pc->n_queries == 0) return 0;   // nothing is read or written
+    const bool bounds = mode == LTPL_PC_INSIDE_BOUNDS;
+    const struct {
+        const void* p;
+        size_t align;
+        bool need;
+        const char* msg;
+    } ptrs[] = {
+        {pc->x, 8, true, "path_coord: pc.x must be set and 8-byte aligned"},
+        {pc->y, 8, true, "path_coord: pc.y must be set and 8-byte aligned"},
+        {pc->pos, 8, true, "path_coord: pc.pos must be set and 8-byte aligned"},
+        {pc->x2, 8, bounds, "path_coord: pc.x2 must be set and 8-byte aligned (LTPL_PC_INSIDE_BOUNDS)"},
+        {pc->y2, 8, bounds, "path_coord: pc.y2 must be set and 8-byte aligned (LTPL_PC_INSIDE_BOUNDS)"},
+        {pc->s, 8, mode == LTPL_PC_S_COORD, "path_coord: pc.s must be set (LTPL_PC_S_COORD) and 8-byte aligned"},
+        {pc->closest, 4, mode <= LTPL_PC_S_INDEX,
+         "path_coord: pc.closest must be set (LTPL_PC_S_COORD, LTPL_PC_S_INDEX) and 4-byte aligned"},
+        {pc->idx, 4, mode == LTPL_PC_CLOSEST, "path_coord: pc.idx must be set (LTPL_PC_CLOSEST) and 4-byte aligned"},
+        {pc->inside, 1, bounds, "path_coord: pc.inside must be set (LTPL_PC_INSIDE_BOUNDS)"},
+        {pc->s_array, 8, false, "path_coord: pc.s_array must be 8-byte aligned"},
+        {pc->n_pts, 4, false, "path_coord: pc.n_pts must be 4-byte aligned"},
+    };
+    for (const auto& a : ptrs)
+        if ((a.need && !a.p) || (a.p && misaligned(a.p, a.align))) return fail(a.msg);
+    if (pc->pt_s < 1) return fail("path_coord: pc.pt_s must be >= 1");
+    if (pc->line_s != 0 && pc->line_s < (m - 1) * pc->pt_s + 1)
+        return fail("path_coord: pc.line_s must be 0 (a shared line) or >= (m_points - 1) pt_s + 1");
+    if (bounds && pc->pt2_s < 1) return fail("path_coord: pc.pt2_s must be >= 1");
+    if (bounds && pc->line2_s != 0 && pc->line2_s < (m - 1) * pc->pt2_s + 1)
+        return fail("path_coord: pc.line2_s must be 0 (a shared line) or >= (m_points - 1) pt2_s + 1");
+    if (mode == LTPL_PC_S_COORD && pc->s_array) {
+        if (pc->s_array_es < 1) return fail("path_coord: pc.s_array_es must be >= 1");
+        if (pc->s_array_s < (m - 1) * pc->s_array_es + 1 && !(pc->s_array_s == 0 && pc->line_s == 0))
+            return fail("path_coord: pc.s_array_s must be >= (m_points - 1) s_array_es + 1 (0 only with a shared line)");
+    }
+    if (pc->pos_s[0] < 0 || pc->pos_s[1] < 1) return fail("path_coord: pc.pos_s must be >= 0 (queries) and >= 1 (x to y)");
+    using Fn = void (*)(const LtplPathCoord);
+    static const Fn kFns[4] = {k_pathcoord<LTPL_PC_S_COORD>, k_pathcoord<LTPL_PC_S_INDEX>, k_pathcoord<LTPL_PC_CLOSEST>,
+                               k_pathcoord<LTPL_PC_INSIDE_BOUNDS>};
+    kFns[mode]<<<(unsigned)(((int64_t)pc->n_queries + PC_WARPS - 1) / PC_WARPS), PC_WARPS * 32, 0, static_cast<cudaStream_t>(stream)>>>(*pc);
+    return check_launch("k_pathcoord");
 }
 
 int ltpl_stage_inputs_batch(const LtplDims* dm, const LtplBuffers* bf, const LtplStageSrc* src, void* stream) {

@@ -314,16 +314,17 @@ __device__ __forceinline__ ArgMinD warp_argmin(double v, int i) {
     return r;
 }
 
-// np.argmin of squared distances between pos and n points (closest_path_index.py:24-30, GIE:41-42, GB:341-345)
-__device__ __noinline__ ArgMinD warp_closest_point(const double2* __restrict__ pts, int n, double px, double py,
-                                                      int lane) {
+// np.argmin of squared distances between pos and the n points pt(i) of a gather (closest_path_index.py:24-30, GIE:41-42,
+// GB:341-345).  A NaN or infinite distance is never taken: without a finite one the index is 0x7fffffff.
+template <class PT>
+__device__ __forceinline__ ArgMinD closest_point_scan(PT pt, int n, double px, double py, int lane) {
     double bv = LTPL_INF;
     int bi = 0x7fffffff;
     #pragma unroll 1
     for (int i0 = lane; i0 < n; i0 += 128) {  // four loads in flight per lane; candidates still visited in index order
         double2 p[4];
 #pragma unroll
-        for (int u = 0; u < 4; ++u) p[u] = pts[min(i0 + 32 * u, n - 1)];
+        for (int u = 0; u < 4; ++u) p[u] = pt(min(i0 + 32 * u, n - 1));
 #pragma unroll
         for (int u = 0; u < 4; ++u) {
             const int i = i0 + 32 * u;
@@ -335,6 +336,10 @@ __device__ __noinline__ ArgMinD warp_closest_point(const double2* __restrict__ p
         }
     }
     return warp_argmin(bv, bi);
+}
+__device__ __noinline__ ArgMinD warp_closest_point(const double2* __restrict__ pts, int n, double px, double py,
+                                                      int lane) {
+    return closest_point_scan([pts](int i) { return pts[i]; }, n, px, py, lane);
 }
 
 // the same argmin for one of the lattice's own polylines: the grid cell of (px, py) bounds the nearest vertex (and every
@@ -408,6 +413,15 @@ __device__ __forceinline__ int lanes_closest_point(const LatDev& lt, const int* 
     return res;
 }
 
+// get_s_coord.py:70-75: distance from a to the foot of the perpendicular from (px, py) on the line a -> b
+__device__ __forceinline__ double foot_ds(const double2& a, const double2& b, double px, double py) {
+    const double bax = b.x - a.x, bay = b.y - a.y;
+    const double t = __ddiv_rn(__dadd_rn(__dmul_rn(px - a.x, bax), __dmul_rn(py - a.y, bay)), __dadd_rn(sq_rn(bax), sq_rn(bay)));
+    const double sx = __dadd_rn(a.x, __dmul_rn(t, bax));
+    const double sy = __dadd_rn(a.y, __dmul_rn(t, bay));
+    return sqrt(__dadd_rn(sq_rn(a.x - sx), sq_rn(a.y - sy)));
+}
+
 // get_s_coord.py:8-99 behind the nearest vertex nb, on a CLOSED polyline with explicit s_array (s_array[0] <= 0.05, i.e.
 // no leading-zero insertion): neighbour choice by the larger angle (:48-58), foot of the perpendicular, s; per lane
 __device__ __forceinline__ double s_coord_from_vertex(const double2* __restrict__ pts, const double* __restrict__ s_arr,
@@ -427,11 +441,39 @@ __device__ __forceinline__ double s_coord_from_vertex(const double2* __restrict_
         b = p2;
         sbase = s_arr[nb];
     }
-    const double bax = b.x - a.x, bay = b.y - a.y;
-    const double t = __ddiv_rn(__dadd_rn(__dmul_rn(px - a.x, bax), __dmul_rn(py - a.y, bay)), __dadd_rn(sq_rn(bax), sq_rn(bay)));
-    const double sx = __dadd_rn(a.x, __dmul_rn(t, bax));
-    const double sy = __dadd_rn(a.y, __dmul_rn(t, bay));
-    return __dadd_rn(sbase, sqrt(__dadd_rn(sq_rn(a.x - sx), sq_rn(a.y - sy))));
+    return __dadd_rn(sbase, foot_ds(a, b, px, py));
+}
+
+// check_inside_bounds.py:36-57 once the centre-line pair (i0, i1) is known (c0, c1 its points; gathers b1(i), b2(i) of
+// the bounds; warp-collective): np.linspace(a, b) with 50 points, y[k] = k * ((b - a) / 49) + a, y[49] = b; the nearest
+// of the centre line's (first minimum), then the track width against the distances to both bounds
+template <class PB1, class PB2>
+__device__ __forceinline__ bool inside_from_pair(double2 c0, double2 c1, PB1 b1, PB2 b2, int i0, int i1, double px,
+                                                 double py, int lane) {
+    double stx = __ddiv_rn(c1.x - c0.x, 49.0), sty = __ddiv_rn(c1.y - c0.y, 49.0);
+    double bv = LTPL_INF;
+    int bi = 0x7fffffff;
+    #pragma unroll 1
+    for (int k = lane; k < 50; k += 32) {
+        double cx = (k == 49) ? c1.x : __dadd_rn(__dmul_rn((double)k, stx), c0.x);
+        double cy = (k == 49) ? c1.y : __dadd_rn(__dmul_rn((double)k, sty), c0.y);
+        double d = dist2_rn(cx, cy, px, py);
+        if (d < bv) {
+            bv = d;
+            bi = k;
+        }
+    }
+    ArgMinD m = warp_argmin(bv, bi);
+    int k = m.i;
+    double2 u0 = b1(i0), u1 = b1(i1), w0 = b2(i0), w1 = b2(i1);
+    double b1x = (k == 49) ? u1.x : __dadd_rn(__dmul_rn((double)k, __ddiv_rn(u1.x - u0.x, 49.0)), u0.x);
+    double b1y = (k == 49) ? u1.y : __dadd_rn(__dmul_rn((double)k, __ddiv_rn(u1.y - u0.y, 49.0)), u0.y);
+    double b2x = (k == 49) ? w1.x : __dadd_rn(__dmul_rn((double)k, __ddiv_rn(w1.x - w0.x, 49.0)), w0.x);
+    double b2y = (k == 49) ? w1.y : __dadd_rn(__dmul_rn((double)k, __ddiv_rn(w1.y - w0.y, 49.0)), w0.y);
+    double d_track_2 = dist2_rn(b1x, b1y, b2x, b2y);
+    double d_b1_2 = dist2_rn(b1x, b1y, px, py);
+    double d_b2_2 = dist2_rn(b2x, b2y, px, py);
+    return !(d_b1_2 > d_track_2 || d_b2_2 > d_track_2);
 }
 
 // check_inside_bounds.py:26-59 (warp-collective)
@@ -453,32 +495,8 @@ __device__ __noinline__ bool inside_bounds(const LatDev& lt, double px, double p
             i1 = idx2;
         }
     }
-    // np.linspace(a, b) with 50 points: y[k] = k * ((b - a) / 49) + a, y[49] = b
-    double2 c0 = lt.center[i0], c1 = lt.center[i1];
-    double stx = __ddiv_rn(c1.x - c0.x, 49.0), sty = __ddiv_rn(c1.y - c0.y, 49.0);
-    double bv = LTPL_INF;
-    int bi = 0x7fffffff;
-    #pragma unroll 1
-    for (int k = lane; k < 50; k += 32) {
-        double cx = (k == 49) ? c1.x : __dadd_rn(__dmul_rn((double)k, stx), c0.x);
-        double cy = (k == 49) ? c1.y : __dadd_rn(__dmul_rn((double)k, sty), c0.y);
-        double d = dist2_rn(cx, cy, px, py);
-        if (d < bv) {
-            bv = d;
-            bi = k;
-        }
-    }
-    ArgMinD m = warp_argmin(bv, bi);
-    int k = m.i;
-    double2 u0 = lt.bound1[i0], u1 = lt.bound1[i1], w0 = lt.bound2[i0], w1 = lt.bound2[i1];
-    double b1x = (k == 49) ? u1.x : __dadd_rn(__dmul_rn((double)k, __ddiv_rn(u1.x - u0.x, 49.0)), u0.x);
-    double b1y = (k == 49) ? u1.y : __dadd_rn(__dmul_rn((double)k, __ddiv_rn(u1.y - u0.y, 49.0)), u0.y);
-    double b2x = (k == 49) ? w1.x : __dadd_rn(__dmul_rn((double)k, __ddiv_rn(w1.x - w0.x, 49.0)), w0.x);
-    double b2y = (k == 49) ? w1.y : __dadd_rn(__dmul_rn((double)k, __ddiv_rn(w1.y - w0.y, 49.0)), w0.y);
-    double d_track_2 = dist2_rn(b1x, b1y, b2x, b2y);
-    double d_b1_2 = dist2_rn(b1x, b1y, px, py);
-    double d_b2_2 = dist2_rn(b2x, b2y, px, py);
-    return !(d_b1_2 > d_track_2 || d_b2_2 > d_track_2);
+    return inside_from_pair(lt.center[i0], lt.center[i1], [&lt](int i) { return lt.bound1[i]; },
+                            [&lt](int i) { return lt.bound2[i]; }, i0, i1, px, py, lane);
 }
 
 // check_inside_bounds.py:26-59 behind the nearest centre-line vertex nb: per lane.  The argmin over the 50 linspace points

@@ -447,29 +447,35 @@ class VelocityPlanner(object):
 def _host_arrays(kappa, n_pts, **arrays) -> dict:
     """host checks shared by the NumPy paths: kappa [N >= 1][P >= 2], n_pts (integers in [2, P]) and every other array
     numeric and not a tensor; returns contiguous float64 arrays (n_pts int32; a loc_gg tuple and None pass through)"""
-    def host(a, name, dtype=np.float64):
-        if isinstance(a, torch.Tensor):
-            raise ValueError("%s: NumPy arrays and tensors cannot be mixed in one call" % name)
-        a = np.asarray(a)
-        if a.dtype.kind not in "iuf":
-            raise ValueError("%s: a numeric array, got %s" % (name, a.dtype))
-        return np.ascontiguousarray(a, dtype=dtype)
-
-    kappa = host(kappa, "kappa")
+    kappa = _host(kappa, "kappa")
     if kappa.ndim != 2 or kappa.shape[0] < 1 or kappa.shape[1] < 2:
         raise ValueError("kappa must be [N >= 1][P >= 2], got %s" % (kappa.shape,))
-    if n_pts is not None:
-        h = np.asarray(n_pts)
-        if h.dtype.kind not in "iu" or h.shape != (kappa.shape[0],):
-            raise ValueError("n_pts: an integer array [%d], got %s" % (kappa.shape[0], _describe(n_pts)))
-        if np.any(h < 2) or np.any(h > kappa.shape[1]):
-            raise ValueError("n_pts: every length must be in [2, %d], got %d .. %d"
-                             % (kappa.shape[1], h.min(), h.max()))
-        n_pts = host(h, "n_pts", np.int32)
-    out = dict(kappa=kappa, n_pts=n_pts)
+    out = dict(kappa=kappa, n_pts=_host_lengths(n_pts, kappa.shape[0], kappa.shape[1]))
     for name, a in arrays.items():
-        out[name] = a if a is None or (name == "loc_gg" and isinstance(a, tuple)) else host(a, name)
+        out[name] = a if a is None or (name == "loc_gg" and isinstance(a, tuple)) else _host(a, name)
     return out
+
+
+def _host(a, name, dtype=np.float64):
+    """a numeric host array (not a tensor) as a contiguous array of dtype"""
+    if isinstance(a, torch.Tensor):
+        raise ValueError("%s: NumPy arrays and tensors cannot be mixed in one call" % name)
+    a = np.asarray(a)
+    if a.dtype.kind not in "iuf":
+        raise ValueError("%s: a numeric array, got %s" % (name, a.dtype))
+    return np.ascontiguousarray(a, dtype=dtype)
+
+
+def _host_lengths(n_pts, n, p):
+    """host lengths n_pts: None, or integers [n] in [2, p] as contiguous int32"""
+    if n_pts is None:
+        return None
+    h = np.asarray(n_pts)
+    if h.dtype.kind not in "iu" or h.shape != (n,):
+        raise ValueError("n_pts: an integer array [%d], got %s" % (n, _describe(n_pts)))
+    if np.any(h < 2) or np.any(h > p):
+        raise ValueError("n_pts: every length must be in [2, %d], got %d .. %d" % (p, h.min(), h.max()))
+    return _host(h, "n_pts", np.int32)
 
 
 def check_follow_args(len_veh, control_type, control_params, glob_rl):

@@ -434,6 +434,39 @@ typedef struct LtplBrakePrefix {
                                /* gives a row of NaN, n_prefix = pref_idx = -1, vel_start NaN and leaves old_gg_scale[i]  */
 } LtplBrakePrefix;
 
+/* Positions on polylines (ltpl_path_coord_batch): the reference's helpers get_s_coord (get_s_coord.py:8-99),            */
+/* closest_path_index (closest_path_index.py:4-32, n_closest = 1) and check_inside_bounds (check_inside_bounds.py:7-59)   */
+/* for n_queries positions at once, query i on line row i (or on one line shared by all).  Every decision is taken in     */
+/* float64 with NumPy's operation order; the nearest point is the first minimum (argpartition's tie order is undefined). */
+/* Arrays are DEVICE pointers; strides are in elements.  The struct carries its own size, as LtplVelPlan does.  A query  */
+/* whose length is out of range, whose position is not finite or whose row has no point at a finite distance is invalid: */
+/* s = NaN, closest = (-2, -2), idx = -1, inside = -1.                                                                   */
+#define LTPL_PC_S_COORD       0 /* get_s_coord: s and closest                                                            */
+#define LTPL_PC_S_INDEX       1 /* get_s_coord(only_index=True): closest; s (optional) NaN                               */
+#define LTPL_PC_CLOSEST       2 /* closest_path_index: idx                                                               */
+#define LTPL_PC_INSIDE_BOUNDS 3 /* check_inside_bounds(bound1 = x / y, bound2 = x2 / y2): inside                        */
+typedef struct LtplPathCoord {
+    int32_t struct_bytes;      /* sizeof(LtplPathCoord) as the caller compiled it; anything else is refused              */
+    int32_t mode;              /* LTPL_PC_*                                                                              */
+    int32_t closed;            /* get_s_coord's closed (S_COORD, S_INDEX); INSIDE_BOUNDS is always closed               */
+    int32_t n_queries;         /* >= 0                                                                                   */
+    int32_t m_points;          /* >= 2 points per row                                                                    */
+    const double* x;           const double* y;  /* point j of row i at x[i * line_s + j * pt_s] (and y)                 */
+    int64_t line_s, pt_s;      /* row stride (0: one line shared by every query, else >= (m_points - 1) pt_s + 1),     */
+                               /* point stride >= 1                                                                      */
+    const double* x2;          const double* y2; /* bound2 (INSIDE_BOUNDS only), the same layout rules                   */
+    int64_t line2_s, pt2_s;
+    const double* s_array;     int64_t s_array_s; /* S_COORD: [n_queries][m_points] the line's s values, element j of  */
+    int64_t s_array_es;        /* row i at s_array[i * s_array_s + j * s_array_es]: element stride >= 1, row stride     */
+                               /* >= (m_points - 1) s_array_es + 1 (0 with a shared line); NULL: cumulated chord lengths */
+    const double* pos;         int64_t pos_s[2];  /* [n_queries][2]; pos_s[0] >= 0, pos_s[1] >= 1                      */
+    const int32_t* n_pts;      /* [n_queries] points of each row, 2 <= n <= m_points; NULL: m_points each                */
+    double* s;                 /* [n_queries] S_COORD (NaN where the reference raises); S_INDEX: NULL or NaN written     */
+    int32_t* closest;          /* [n_queries][2] S_COORD, S_INDEX: closest_indexes (-1: NumPy's last element)            */
+    int32_t* idx;              /* [n_queries] CLOSEST                                                                    */
+    int8_t* inside;            /* [n_queries] INSIDE_BOUNDS: 1 inside, 0 outside                                         */
+} LtplPathCoord;
+
 /* Scenario inputs that already live on the device (ltpl_stage_inputs_batch): DEVICE pointers and strides, in elements,  */
 /* of the caller's arrays, read through their strides, so column slices and wider rows need no copy.  Scalars have one   */
 /* stride, [B][..] arrays one per dimension.                                                                             */
@@ -536,6 +569,9 @@ int ltpl_vel_follow_batch(const LtplParams* prm, const LtplVelFollow* vf, void* 
 /* brake prefixes to a lowered vel_max (LtplBrakePrefix), in ONE launch on the stream; bad arguments are refused before  */
 /* it, with the field named                                                                                              */
 int ltpl_brake_prefix_batch(const LtplParams* prm, const LtplBrakePrefix* bp, void* stream);
+/* positions on polylines (LtplPathCoord), in ONE launch on the stream (none for n_queries = 0); bad arguments are      */
+/* refused before it, with the field named; with n_queries = 0 no pointer is read                                     */
+int ltpl_path_coord_batch(const LtplPathCoord* pc, void* stream);
 /* scenario inputs from device arrays, in ONE launch on the stream (k_stage): writes the input buffers of `buf` (pos,     */
 /* heading, vel, vel_est, n_obj, obj, zone_sel, n_pred, obj_pred; their const marks what the tick kernels do) with the   */
 /* bytes a host copy of the same arrays writes: obj slots k >= k_src and obj_pred behind the given points zero, n_pred   */

@@ -125,3 +125,20 @@ for gg, n_pts in ((fgg, np.random.default_rng(9).integers(2, 91, size=70)), ((5.
     bx, bn, bi, bs = bv.check_brake_prefix(bplan, brng.uniform(10.0, 60.0, size=(70, 4)), fi["kappa"], fi["el"], gg,
                                            bold, n_course=brng.integers(0, 5, size=70), n_pts=n_pts)
     print("brake prefix mean", float(np.mean(bx)), "braking", int((bi > 0).sum()), "n_prefix", int(bn.sum()))
+
+# positions on polylines: each mode on ragged per-query rows with invalid ones (device lengths out of range, a NaN
+# position, an all-NaN row) and on a shared line
+from graphbasedlocaltrajectoryplanner_b200 import pathcoord  # noqa: E402
+prng = np.random.default_rng(10)
+pts = torch.as_tensor(np.cumsum(prng.uniform(0.1, 2.0, size=(40, 60, 2)), axis=1), device="cuda:0")
+ppos = pts[:, 20, :] + torch.as_tensor(prng.normal(0.0, 1.0, size=(40, 2)), device="cuda:0")
+ppos[3, 0] = float("nan")
+pts[5] = float("nan")
+pn = torch.as_tensor(prng.integers(2, 61, size=40), dtype=torch.int32, device="cuda:0")
+pn[0], pn[1], pn[2] = 0, 1, 61
+ps, pci = pathcoord.get_s_coord(pts, ppos, n_pts=pn, closed=True)
+ps2, _ = pathcoord.get_s_coord(pts, ppos, s_array=pts[:, :, 0], n_pts=pn)
+pidx = pathcoord.closest_path_index(pts[0], ppos)
+pin = pathcoord.check_inside_bounds(pts, pts + 2.0, ppos, n_pts=pn)
+print("path coord s", float(torch.nansum(ps)), float(torch.nansum(ps2)), "idx", int(pidx.sum()), "inside",
+      int(pin.sum()), "pairs", int(pci.sum()))
